@@ -33,6 +33,7 @@ namespace tc {
 struct ChainLayer {                 // device copy of one layer (64-byte aligned array)
     const float* in;
     const float* bias;
+    const float* wscale;            // per output channel, null = 1
     const float* res;
     float* out;
     int H, W, Cin, ldin;
@@ -100,7 +101,8 @@ __device__ __forceinline__ unsigned long long gtime() {
 }
 
 // Epilogue of one work item straight from the accumulator fragment: a raw partial (split-K, not the last split) or the
-// finished tile (partials of the other splits in split order + own sum, bias, residual, activation).
+// finished tile (partials of the other splits in split order + own sum, times wscale, bias, residual, activation).  The
+// scale is applied to the finished sum only: the raw partials are unscaled.
 template <int BN>
 __device__ __forceinline__ void chain_epilogue(const ChainArgs& a, const ChainLayer& L, const ChainTile& t, const float* acc) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -129,9 +131,10 @@ __device__ __forceinline__ void chain_epilogue(const ChainArgs& a, const ChainLa
                 o.x = p.x + o.x; o.y = p.y + o.y;
             }
             const float2 b2 = (L.bias && !noload) ? *reinterpret_cast<const float2*>(L.bias + n) : make_float2(0.f, 0.f);
+            const float2 s2 = (L.wscale && !noload) ? *reinterpret_cast<const float2*>(L.wscale + n) : make_float2(1.f, 1.f);
             const float2 r2 = (L.res && !noload) ? *reinterpret_cast<const float2*>(L.res + (size_t)m * L.ldres + n)
                                                  : make_float2(0.f, 0.f);
-            o.x += b2.x; o.y += b2.y;
+            o.x = fmaf(o.x, s2.x, b2.x); o.y = fmaf(o.y, s2.y, b2.y);      // exact product: rounds like o * s + b
             o.x += r2.x; o.y += r2.y;
             o.x = apply_act(o.x, L.act); o.y = apply_act(o.y, L.act);
             if (!nostore) *reinterpret_cast<float2*>(L.out + (size_t)m * L.ldout + n) = o;
@@ -263,6 +266,7 @@ struct aotb_chain_layer {
     const void* wh;
     const void* wl;
     const float* bias;
+    const float* wscale;
     const float* res;
     float* out;
     int H, W, Cin, ldin, Cout, ldout, ldres, KH, KW, stride, pad, act, in_layer, res_layer;
@@ -286,7 +290,7 @@ int plan_chain(const aotb_chain_layer* ls, int n, ChainPlan& P) {
         AOTB_REQUIRE(l.ldin % 4 == 0 && l.ldout % 4 == 0 && (!l.res || l.ldres % 4 == 0), "aotb_conv_chain: layer %d: strides", i);
         AOTB_REQUIRE(l.in_layer < i && l.res_layer < i, "aotb_conv_chain: layer %d: producers must come earlier in the chain", i);
         tc::ChainLayer d{};
-        d.in = l.in; d.bias = l.bias; d.res = l.res; d.out = l.out;
+        d.in = l.in; d.bias = l.bias; d.wscale = l.wscale; d.res = l.res; d.out = l.out;
         d.H = l.H; d.W = l.W; d.Cin = l.Cin; d.ldin = l.ldin;
         d.Ho = (l.H + 2 * l.pad - l.KH) / l.stride + 1;
         d.Wo = (l.W + 2 * l.pad - l.KW) / l.stride + 1;

@@ -1,7 +1,11 @@
 // Implicit-GEMM convolution / linear layer on the Hopper tensor cores (wgmma + TMA + mbarrier), NHWC fp32 in / fp32 out,
-// fp32-faithful through the split-fp16 ("fp16x2") scheme of lt_attn_tc.cu.
+// through the split-fp16 ("fp16x2") scheme of lt_attn_tc.cu.
 //
-//   out[m][n] = act( sum_k A(m,k) * W[k][n] + bias[n] + res[m][n] )      m -> (b, oy, ox), k -> (ky, kx, ci)
+//   out[m][n] = act( wscale[n] * sum_k A(m,k) * W'[k][n] + bias[n] + res[m][n] )      m -> (b, oy, ox), k -> (ky, kx, ci)
+//
+// The weights arrive normalised per output channel (ops.split_fp16_scaled): column n holds w * 2^e_n and the finish
+// multiplies the accumulator by wscale[n] = 2^-e_n, an exact operation, so the split keeps its relative precision for
+// channels of any magnitude.
 //
 // Same reference sites as conv_igemm.cu (resnet.py:34-54,140-157 with FrozenBatchNorm2d folded,
 // aot.py:19-21,83, fpn.py:34-58, every nn.Linear of transformer.py:321-367,582-665).  Eligibility:
@@ -20,6 +24,7 @@ namespace tc {
 struct ConvTcArgs {
     const float* in;
     const float* bias;
+    const float* wscale;   // per output channel, null = 1
     const float* res;
     float* out;
     int B, H, W, Cin, ldin;
@@ -50,6 +55,7 @@ __device__ __forceinline__ void conv_finish_tile(const ConvTcArgs& a, const uint
     const int c = (tid % C4) * 4, n = n0 + c;
     const int r0 = zrank * ROWS + tid / C4;
     const float4 b4 = a.bias ? __ldg(reinterpret_cast<const float4*>(a.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 s4 = a.wscale ? __ldg(reinterpret_cast<const float4*>(a.wscale + n)) : make_float4(1.f, 1.f, 1.f, 1.f);
     const float* lbase = reinterpret_cast<const float*>(smem) + r0 * LD + c;
     const uint32_t sbase = smem_u32(lbase);
 #pragma unroll 1
@@ -73,7 +79,8 @@ __device__ __forceinline__ void conv_finish_tile(const ConvTcArgs& a, const uint
             float4 o = v[b][0];
 #pragma unroll
             for (int z = 1; z < S; ++z) { o.x += v[b][z].x; o.y += v[b][z].y; o.z += v[b][z].z; o.w += v[b][z].w; }
-            o.x += b4.x; o.y += b4.y; o.z += b4.z; o.w += b4.w;
+            // o * s is exact (s is a power of two), so the fma rounds like o * s + b
+            o.x = fmaf(o.x, s4.x, b4.x); o.y = fmaf(o.y, s4.y, b4.y); o.z = fmaf(o.z, s4.z, b4.z); o.w = fmaf(o.w, s4.w, b4.w);
             o.x += rs[b].x; o.y += rs[b].y; o.z += rs[b].z; o.w += rs[b].w;
             o.x = apply_act(o.x, a.act); o.y = apply_act(o.y, a.act);
             o.z = apply_act(o.z, a.act); o.w = apply_act(o.w, a.act);
@@ -88,13 +95,14 @@ __device__ __forceinline__ void conv_finish_tile(const ConvTcArgs& a, const uint
 // K loop), and inside the loop the residual rows of batch k+1 are requested before batch k is computed and stored.  The staging
 // tile is read with ld.shared so that the compiler does not have to order those reads behind the global stores.
 template <int BN>
-struct FinishPre { float4 b4; float4 rs[8]; };
+struct FinishPre { float4 b4, s4; float4 rs[8]; };
 
 template <int BN>
 __device__ __forceinline__ void finish_prefetch(const ConvTcArgs& a, int tid, int m0, int n0, FinishPre<BN>& pre) {
     constexpr int C4 = BN / 4, RSTEP = 256 / C4;
     const int n = n0 + (tid % C4) * 4, r0 = tid / C4;
     pre.b4 = a.bias ? __ldg(reinterpret_cast<const float4*>(a.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    pre.s4 = a.wscale ? __ldg(reinterpret_cast<const float4*>(a.wscale + n)) : make_float4(1.f, 1.f, 1.f, 1.f);
 #pragma unroll
     for (int b = 0; b < 8; ++b) {
         const int m = m0 + r0 + b * RSTEP;
@@ -131,7 +139,8 @@ __device__ __forceinline__ void conv_finish_tile_pre(const ConvTcArgs& a, const 
 #pragma unroll
         for (int b = 0; b < B; ++b) {
             float4 o = v[b];
-            o.x += pre.b4.x; o.y += pre.b4.y; o.z += pre.b4.z; o.w += pre.b4.w;
+            o.x = fmaf(o.x, pre.s4.x, pre.b4.x); o.y = fmaf(o.y, pre.s4.y, pre.b4.y);
+            o.z = fmaf(o.z, pre.s4.z, pre.b4.z); o.w = fmaf(o.w, pre.s4.w, pre.b4.w);
             o.x += rs[b].x; o.y += rs[b].y; o.z += rs[b].z; o.w += rs[b].w;
             o.x = apply_act(o.x, a.act); o.y = apply_act(o.y, a.act);
             o.z = apply_act(o.z, a.act); o.w = apply_act(o.w, a.act);
@@ -322,18 +331,20 @@ extern "C" int aotb_set_conv_tiling(int mode) {
     return AOTB_OK;
 }
 
-// wh / wl: pre-split weights [Cout][Kpad] fp16 (K = KH*KW*Cin ordered (ky,kx,ci), zero-padded to a multiple of 64).
-extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* wl, const float* bias, const float* res,
-                                   float* out, int B, int H, int W, int Cin, int ldin, int Cout, int ldout, int ldres,
+// wh / wl: pre-split weights [Cout][Kpad] fp16 (K = KH*KW*Cin ordered (ky,kx,ci), zero-padded to a multiple of 64);
+// wscale [Cout]: per-channel factor of the accumulator (null = 1).
+extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* wl, const float* bias, const float* wscale,
+                                   const float* res, float* out, int B, int H, int W, int Cin, int ldin, int Cout, int ldout, int ldres,
                                    int KH, int KW, int stride, int pad, int act, void* workspace, size_t workspace_bytes,
                                    void* stream) {
     AOTB_REQUIRE(in && wh && wl && out, "aotb_conv2d_nhwc_tc: null pointer");
     AOTB_REQUIRE(Cin % 4 == 0 && Cout % 64 == 0, "aotb_conv2d_nhwc_tc: Cin must be a multiple of 4, Cout of 64");
     AOTB_REQUIRE(ldin % 4 == 0 && ldout % 4 == 0 && (!res || ldres % 4 == 0) && ((uintptr_t)in % 16 == 0) &&
-                     ((uintptr_t)out % 16 == 0) && (!res || (uintptr_t)res % 16 == 0) && (!bias || (uintptr_t)bias % 16 == 0),
+                     ((uintptr_t)out % 16 == 0) && (!res || (uintptr_t)res % 16 == 0) && (!bias || (uintptr_t)bias % 16 == 0) &&
+                     (!wscale || (uintptr_t)wscale % 16 == 0),
                  "aotb_conv2d_nhwc_tc: 16-byte alignment required");
     tc::ConvTcArgs a;
-    a.in = in; a.bias = bias; a.res = res; a.out = out;
+    a.in = in; a.bias = bias; a.wscale = wscale; a.res = res; a.out = out;
     a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.ldin = ldin;
     a.Ho = (H + 2 * pad - KH) / stride + 1;
     a.Wo = (W + 2 * pad - KW) / stride + 1;

@@ -45,7 +45,8 @@ def _nhwc_ld(x):
     return ld
 
 
-# fp32 weight (by data_ptr) -> (wh, wl) split-fp16 [Cout, K] copies for the tensor-core conv (registered by plan.py)
+# fp32 weight (by data_ptr) -> (wh, wl, wscale, w): split-fp16 [Cout, K] copies for the tensor-core conv and their
+# per-channel scale (None = 1), registered by plan.py
 _TC_WEIGHTS = {}
 CONV_IMPL = os.environ.get("AOTB_CONV_IMPL", "tc")     # "tc" (wgmma, fp16x2 split) | "simt" (fp32 CUDA cores)
 
@@ -80,12 +81,13 @@ def _tc_workspace(device):
     return ws
 
 
-def register_tc_weights(w, wh, wl):
-    _TC_WEIGHTS[w.data_ptr()] = (wh, wl, w)     # keep w alive so the pointer key stays unique
+def register_tc_weights(w, wh, wl, wscale=None):
+    _TC_WEIGHTS[w.data_ptr()] = (wh, wl, wscale, w)     # keep w alive so the pointer key stays unique
 
 
 def split_fp16(w_kn):
-    """fp32 [K, N] -> (hi, lo) fp16 [N, Kpad] (K zero-padded to a multiple of 64) with hi + lo ~= w to 2^-22."""
+    """fp32 [K, N] -> (hi, lo) fp16 [N, Kpad] (K zero-padded to a multiple of 64) with hi + lo ~= w to 2^-22 relative,
+    but never closer than the fp16 subnormal spacing of lo (2^-25 absolute): see split_fp16_scaled."""
     K = w_kn.shape[0]
     wt = w_kn.t().contiguous()
     if K % 64:
@@ -93,6 +95,30 @@ def split_fp16(w_kn):
     hi = wt.half()
     lo = (wt - hi.float()).half()
     return hi.contiguous(), lo.contiguous()
+
+
+def weight_scale_exponents(w_kn):
+    """fp32 [K, N] -> int32 [N]: e_n = 13 - floor(log2 max_k |w[k][n]|), so that 2^13 <= max_k |w[k][n]| 2^e_n < 2^14
+    (0 for an all-zero column; at most 126 so that 2^-e_n stays a normal fp32 number)."""
+    amax = w_kn.abs().amax(dim=0).float()
+    _, ex = torch.frexp(amax)                      # amax = m 2^ex, m in [0.5, 1): floor(log2 amax) = ex - 1
+    e = (14 - ex).clamp(max=126)
+    return torch.where(amax > 0, e, torch.zeros_like(e)).to(torch.int32)
+
+
+def split_fp16_scaled(w_kn):
+    """fp32 [K, N] -> (hi, lo, wscale): split_fp16 of w normalised per output channel, w[:, n] 2^e_n
+    (weight_scale_exponents), and wscale = 2^-e_n fp32 [N].  Both scalings are exact, and the tensor-core finish multiplies
+    the accumulator by wscale: a channel of any magnitude keeps the 2^-22 relative precision of the split instead of
+    hitting the absolute floor of lo."""
+    e = weight_scale_exponents(w_kn)
+    hi, lo = split_fp16(w_kn.float() * _pow2(e))
+    return hi, lo, _pow2(-e)
+
+
+def _pow2(e):
+    """int32 exponents in [-126, 127] -> exact fp32 powers of two (built from the exponent bits)."""
+    return ((e + 127) << 23).to(torch.int32).view(torch.float32)
 
 
 # ---- a chain of tensor-core convs as one persistent dataflow kernel (csrc/conv_chain.cu)
@@ -103,7 +129,7 @@ def _chain_struct():
     import ctypes
 
     class ChainLayer(ctypes.Structure):
-        _fields_ = [(n, ctypes.c_void_p) for n in ("inp", "wh", "wl", "bias", "res", "out")] + \
+        _fields_ = [(n, ctypes.c_void_p) for n in ("inp", "wh", "wl", "bias", "wscale", "res", "out")] + \
                    [(n, ctypes.c_int) for n in ("H", "W", "Cin", "ldin", "Cout", "ldout", "ldres", "KH", "KW", "stride", "pad",
                                                 "act", "in_layer", "res_layer")]
     return ChainLayer
@@ -125,7 +151,7 @@ def conv_chain_layers(layers):
             raise AotbError("conv_chain: batch 1 only")
         a = arr[i]
         a.inp, a.wh, a.wl = x.data_ptr(), t[0].data_ptr(), t[1].data_ptr()
-        a.bias, a.res, a.out = _p(l["bias"]), _p(res), out.data_ptr()
+        a.bias, a.wscale, a.res, a.out = _p(l["bias"]), _p(t[2]), _p(res), out.data_ptr()
         a.H, a.W, a.Cin, a.ldin = H, W, Cin, _nhwc_ld(x)
         a.Cout, a.ldout, a.ldres = out.shape[3], _nhwc_ld(out), (_nhwc_ld(res) if res is not None else 0)
         a.KH = a.KW = l.get("KH", 1)
@@ -177,14 +203,14 @@ class ConvChain:
         return self.program[off:off + self.ntiles * 32].view(torch.int64).view(self.ntiles, 4).cpu()
 
 
-def conv2d_tc(x, wh, wl, bias, out, res=None, KH=1, KW=1, stride=1, pad=0, act=ACT_NONE, stream=None):
-    """Tensor-core conv: x [B,H,W,Cin] fp32, wh/wl [Cout, KH*KW*Cin] fp16."""
-    _chk(x, bias, out, res)
+def conv2d_tc(x, wh, wl, bias, out, res=None, KH=1, KW=1, stride=1, pad=0, act=ACT_NONE, stream=None, wscale=None):
+    """Tensor-core conv: x [B,H,W,Cin] fp32, wh/wl [Cout, KH*KW*Cin] fp16, wscale fp32 [Cout] or None (= 1)."""
+    _chk(x, bias, out, res, wscale)
     B, H, W, Cin = x.shape
     Cout = wh.shape[0]
     ws = _tc_workspace(x.device)
     with _ConvProbe(2.0 * out.shape[0] * out.shape[1] * out.shape[2] * Cout * KH * KW * Cin, stream):
-        check(lib().aotb_conv2d_nhwc_tc(_p(x), wh.data_ptr(), wl.data_ptr(), _p(bias), _p(res), _p(out), B, H, W, Cin,
+        check(lib().aotb_conv2d_nhwc_tc(_p(x), wh.data_ptr(), wl.data_ptr(), _p(bias), _p(wscale), _p(res), _p(out), B, H, W, Cin,
                                         _nhwc_ld(x), Cout, _nhwc_ld(out), _nhwc_ld(res) if res is not None else 0, KH, KW,
                                         stride, pad, act, ws.data_ptr(), ws.numel(), _st(stream)), "aotb_conv2d_nhwc_tc")
     return out
@@ -196,7 +222,7 @@ def conv2d(x, w, bias, out, res=None, KH=1, KW=1, stride=1, pad=0, dil=1, act=AC
         t = _TC_WEIGHTS.get(w.data_ptr())
         if t is not None:
             return conv2d_tc(x, t[0], t[1], bias, out, res=res, KH=KH, KW=KW, stride=stride, pad=pad, act=act,
-                             stream=stream)
+                             stream=stream, wscale=t[2])
     _chk(x, w, bias, out, res)
     B, H, W, Cin = x.shape
     Cout = w.shape[1]
@@ -211,13 +237,13 @@ def linear(x, wt, bias, out, res=None, act=ACT_NONE, stream=None):
     if CONV_IMPL == "tc":
         t = _TC_WEIGHTS.get(wt.data_ptr())
         if t is not None:
-            _chk(x, bias, out, res)
+            _chk(x, bias, out, res, t[2])
             M, K = x.shape
             N = wt.shape[1]
             ws = _tc_workspace(x.device)
             with _ConvProbe(2.0 * M * N * K, stream):
-                check(lib().aotb_conv2d_nhwc_tc(_p(x), t[0].data_ptr(), t[1].data_ptr(), _p(bias), _p(res), _p(out), 1, M, 1,
-                                                K, x.stride(0), N, out.stride(0), res.stride(0) if res is not None else 0,
+                check(lib().aotb_conv2d_nhwc_tc(_p(x), t[0].data_ptr(), t[1].data_ptr(), _p(bias), _p(t[2]), _p(res), _p(out),
+                                                1, M, 1, K, x.stride(0), N, out.stride(0), res.stride(0) if res is not None else 0,
                                                 1, 1, 1, 0, act, ws.data_ptr(), ws.numel(), _st(stream)),
                       "aotb_conv2d_nhwc_tc")
             return out
@@ -241,7 +267,7 @@ def linear_tc(x, wh, wl, bias, out, res=None, act=ACT_NONE, stream=None):
     if wh.shape[1] != K or K % 64 or N % 64 or out.shape[0] != M or out.shape[1] != N:
         raise AotbError(f"linear_tc: shapes x {tuple(x.shape)}, w {tuple(wh.shape)}, out {tuple(out.shape)}")
     ws = _tc_workspace(x.device)
-    check(lib().aotb_conv2d_nhwc_tc(_p(x), wh.data_ptr(), wl.data_ptr(), _p(bias), _p(res), _p(out), 1, M, 1, K,
+    check(lib().aotb_conv2d_nhwc_tc(_p(x), wh.data_ptr(), wl.data_ptr(), _p(bias), None, _p(res), _p(out), 1, M, 1, K,
                                     x.stride(0), N, out.stride(0), res.stride(0) if res is not None else 0, 1, 1, 1, 0,
                                     act, ws.data_ptr(), ws.numel(), _st(stream)), "aotb_conv2d_nhwc_tc")
     return out

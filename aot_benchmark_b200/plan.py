@@ -66,7 +66,8 @@ class Plan:
 
     def _upload(self):
         """Move every packed host tensor hanging off the plan to the device (shared tensors stay shared) and register the
-        split-fp16 [Cout, K] copies of the GEMM-shaped weights under their device pointers."""
+        split-fp16 [Cout, K] copies of the GEMM-shaped weights, normalised per output channel, and their scales under
+        their device pointers."""
         from . import ops
         memo = {}
 
@@ -96,8 +97,8 @@ class Plan:
             e = memo.get(id(w))
             if e is None:
                 continue                                       # e.g. Q / K projections that only live on concatenated
-            wh, wl = ops.split_fp16(w)
-            ops.register_tc_weights(e[1], wh.to(self.device), wl.to(self.device))
+            wh, wl, ws = ops.split_fp16_scaled(w)
+            ops.register_tc_weights(e[1], wh.to(self.device), wl.to(self.device), ws.to(self.device))
             self._tc_keys.append(e[1].data_ptr())
         self._tc_list = []
 

@@ -45,15 +45,21 @@ int aotb_conv2d_nhwc_f32(const float* in, const float* w, const float* bias, con
                          int B, int H, int W, int Cin, int ldin, int Cout, int ldout, int ldres,
                          int KH, int KW, int stride, int pad, int dil, int act, void* stream);
 
-/* Same contract as aotb_conv2d_nhwc_f32 (dilation 1) on the Hopper tensor cores (wgmma), fp32-faithful through split-fp16
- * operands: wh / wl are the weights pre-split as hi = fp16(w), lo = fp16(w - hi), laid out [Cout][KH*KW*Cin] (K-major,
- * K ordered (ky,kx,ci), zero-padded to a multiple of 64); activations are split on the fly.
+/* Same contract as aotb_conv2d_nhwc_f32 (dilation 1) on the Hopper tensor cores (wgmma) through split-fp16 operands:
+ * wh / wl are the weights pre-split as hi = fp16(w'), lo = fp16(w' - hi), laid out [Cout][KH*KW*Cin] (K-major, K ordered
+ * (ky,kx,ci), zero-padded to a multiple of 64); activations are split on the fly.  out = act(wscale * acc + bias + res):
+ * wscale [Cout] (NULL = 1, 16-byte aligned like bias) undoes a per-output-channel power-of-two normalisation
+ * w' = w / wscale (ops.split_fp16_scaled picks 2^13 <= max_k |w'[k][n]| < 2^14).
+ * Precision: lo cannot go below the fp16 subnormal spacing 2^-24, so each split operand x carries an absolute error of up
+ * to 2^-25 on top of a relative 2^-22.  The normalisation takes that floor off the weights, whose products then stay
+ * within ~1e-6 of fp32 for channels of any magnitude.  Activations are split as they come: elements with |x| below about
+ * 2^-3 lose relative precision, and |x| >= 65520 overflows hi (inf).
  * Requires Cin % 4 == 0 and Cout % 64 == 0.  Few-tile deep-K layers run split-K: the 2 / 4 / 8 CTAs of one output
  * tile form a thread-block cluster and sum their partial tiles over distributed shared memory in rank order
  * (deterministic).  `workspace` / `workspace_bytes` are only used by the diagnostic mode of aotb_set_conv_tiling
  * (may be NULL / 0 otherwise). */
-int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* wl, const float* bias, const float* res,
-                        float* out, int B, int H, int W, int Cin, int ldin, int Cout, int ldout, int ldres,
+int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* wl, const float* bias, const float* wscale,
+                        const float* res, float* out, int B, int H, int W, int Cin, int ldin, int Cout, int ldout, int ldres,
                         int KH, int KW, int stride, int pad, int act, void* workspace, size_t workspace_bytes,
                         void* stream);
 
@@ -191,6 +197,7 @@ typedef struct aotb_chain_layer {
     const void* wh;
     const void* wl;
     const float* bias;
+    const float* wscale;      /* per-output-channel factor of the finished sum, as in aotb_conv2d_nhwc_tc (NULL = 1) */
     const float* res;
     float* out;
     int H, W, Cin, ldin, Cout, ldout, ldres, KH, KW, stride, pad, act, in_layer, res_layer;
@@ -214,11 +221,14 @@ int aotb_nearest_resize_f32(const float* in, float* out, int H, int W, int Ho, i
 
 /* Tensor-core long-term attention (wgmma + TMA), AOT head shape H x 32, split-fp16 ("fp16x2")
  * operands: every fp32 value x is stored as hi = fp16(x), lo = fp16(x - hi) in rows [hi(32) | lo(32)].
+ * The operands are not normalised: each element keeps an absolute error floor of 2^-25 (values below about 2^-3 lose
+ * relative precision) and |x| >= 65520 overflows hi.  K and V rows beyond the live key count get probability 0 but still
+ * enter the P V product, so they must be finite (0 * NaN is NaN); Q rows beyond N only affect rows that are not written.
  * networks/layers/attention.py:82-117 called from networks/layers/transformer.py:346 (and :324, Tk = N).
  *   aotb_tc_pack_rows_f16x2: fp32 [rows][ld] -> packed [H][cap][64] at a row offset, values / div first
  *                            (div = T for Q, attention.py:82; 1 for K and V).  Buffers must be zero-filled
  *                            beyond the live rows.
- *   aotb_lt_attn_tc_f16x2  : exact bit 0 set -> S = QhKh + QlKh + QhKl, O = (Ph + Pl)[Vh|Vl] (fp32-faithful);
+ *   aotb_lt_attn_tc_f16x2  : exact bit 0 set -> S = QhKh + QlKh + QhKl, O = (Ph + Pl)[Vh|Vl];
  *                            clear -> S = QhKh, O = Ph[Vh|Vl].  exact bit 2: the mbarrier waits poll instead of
  *                            sleeping (latency experiment; results unchanged).  splits > 1 writes split-KV partials
  *                            for aotb_attn_merge_f32 (splits cut on 128-key boundaries).  dbg (optional) receives S of
