@@ -15,6 +15,9 @@ _MODELS = {
     "aotl": ("aot", "mobilenetv2", [24, 32, 96, 1280], 3, True, 5),
     # configs/models/r50_aotl.py:7-16
     "r50_aotl": ("aot", "resnet50", [256, 512, 1024, 1024], 3, True, 5),
+    # configs/models/r101_aotl.py, rs101_aotl.py
+    "r101_aotl": ("aot", "resnet101", [256, 512, 1024, 1024], 3, True, 5),
+    "rs101_aotl": ("aot", "resnest101", [256, 512, 1024, 1024], 3, True, 5),
     # configs/models/default_deaot.py:9-17 + deaot*.py
     "deaott": ("deaot", "mobilenetv2", [24, 32, 96, 1280], 1, True, 9999),
     "deaots": ("deaot", "mobilenetv2", [24, 32, 96, 1280], 2, True, 9999),

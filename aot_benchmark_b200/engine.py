@@ -223,8 +223,10 @@ class _Encoder:
         st = _cur_stream()
         if P.encoder_name == "resnet50" and ops.CONV_CHAIN and ops.CONV_IMPL == "tc":
             return self._resnet_chain(x, st)
-        if P.encoder_name == "resnet50":
+        if P.encoder_name in ("resnet50", "resnet101"):
             feats = self._resnet(x, st)
+        elif P.encoder_name == "resnest101":
+            feats = self._resnest(x, st)
         elif P.encoder_name == "swin_base":
             feats = self._swin(x, st)
         else:
@@ -258,6 +260,58 @@ class _Encoder:
                     res = cur
                 out = self._buf(f"s{si}o{bi % 2}", (1, ho, wo, b.c3.cout))
                 ops.conv2d(t2, b.c3.w, b.c3.b, out, res=res, act=A_RELU, stream=st)
+                cur, h, w = out, ho, wo
+            feats.append(cur)
+        return feats
+
+    def _resnest(self, x, st):
+        """ResNeSt-101 (resnest/resnet.py:418-435): deep stem, max-pool, then per bottleneck conv1, the radix-2 grouped 3x3 conv
+        as one tensor-core launch per group on channel slices (group g reads channels [g gw/2, (g+1) gw/2) of t1 and writes
+        [g gw, (g+1) gw) of t2), the split attention (pixel reduction + fc1 / fc2 / radix softmax in one launch), the
+        attention-weighted sum of the two splits (with the avd pool fused in the strided first blocks), the avg_down
+        downsample (pool + conv) and conv3 with the residual and ReLU fused: 6 launches per block, 8 in a strided first block."""
+        e = self.plan.enc
+        H, W = x.shape[1], x.shape[2]
+        h, w = self._osz(H, 3, 2, 1), self._osz(W, 3, 2, 1)
+        s0 = self._buf("stem0", (1, h, w, e.stem[0].cout))
+        ops.conv2d(x, e.stem[0].w, e.stem[0].b, s0, KH=3, KW=3, stride=2, pad=1, act=A_RELU, stream=st)
+        s1 = self._buf("stem1", (1, h, w, e.stem[1].cout))
+        ops.conv2d(s0, e.stem[1].w, e.stem[1].b, s1, KH=3, KW=3, pad=1, act=A_RELU, stream=st)
+        s2 = self._buf("stem2", (1, h, w, e.stem[2].cout))
+        ops.conv2d(s1, e.stem[2].w, e.stem[2].b, s2, KH=3, KW=3, pad=1, act=A_RELU, stream=st)
+        h, w = self._osz(h, 3, 2, 1), self._osz(w, 3, 2, 1)
+        cur = self._buf("pool", (1, h, w, s2.shape[3]))
+        ops.maxpool3x3s2(s2, cur, stream=st)
+        ws = self.bufs.get("splat_ws")         # zero-filled once (launch counter), kept for the encoder's lifetime
+        if ws is None:
+            ws = self.bufs["splat_ws"] = ops.splat_workspace(max(b.gw for blocks in e.stages for b in blocks), self.dev)
+        feats = []
+        for si, blocks in enumerate(e.stages):
+            for bi, b in enumerate(blocks):
+                gw, s = b.gw, b.stride
+                ho, wo = (ops.pool2d_size(h, 3, s, 1), ops.pool2d_size(w, 3, s, 1)) if s > 1 else (h, w)
+                t1 = self._buf(f"s{si}b{bi}t1", (1, h, w, gw))
+                ops.conv2d(cur, b.c1.w, b.c1.b, t1, act=A_RELU, stream=st)
+                t2 = self._buf(f"s{si}b{bi}t2", (1, h, w, 2 * gw))
+                for g, cg in enumerate(b.groups):
+                    ops.conv2d(t1[..., g * gw // 2:(g + 1) * gw // 2], cg.w, cg.b, t2[..., g * gw:(g + 1) * gw], KH=3, KW=3,
+                               pad=1, act=A_RELU, stream=st)
+                att = self._buf(f"s{si}b{bi}att", (2 * gw,))
+                ops.splat_attention(t2, b.fc1_w, b.fc1_b, b.fc2_w, b.fc2_b, att, ws, stream=st)
+                comb = self._buf(f"s{si}b{bi}sum", (1, ho, wo, gw))
+                ops.splat_combine(t2, att, comb, pool_stride=s if s > 1 else 0, stream=st)
+                if b.down is not None:
+                    dsrc = cur
+                    if s > 1:                                  # AvgPool2d(s, s, ceil_mode=True, count_include_pad=False)
+                        dsrc = self._buf(f"s{si}dp", (1, ops.pool2d_size(h, s, s, 0, True), ops.pool2d_size(w, s, s, 0, True),
+                                                      cur.shape[3]))
+                        ops.avgpool(cur, dsrc, s, s, 0, ceil_mode=True, count_include_pad=False, stream=st)
+                    res = self._buf(f"s{si}ds", (1, ho, wo, b.down.cout))
+                    ops.conv2d(dsrc, b.down.w, b.down.b, res, stream=st)
+                else:
+                    res = cur
+                out = self._buf(f"s{si}o{bi % 2}", (1, ho, wo, b.c3.cout))
+                ops.conv2d(comb, b.c3.w, b.c3.b, out, res=res, act=A_RELU, stream=st)
                 cur, h, w = out, ho, wo
             feats.append(cur)
         return feats

@@ -73,13 +73,16 @@ def _seq(mods):
 
 
 # ---------------------------------------------------------------- encoders
-def _resnet50():
-    # resnet.py:57-138: Bottleneck [3,4,6], stride on conv2, layer4 dropped
+RESNET_LAYERS = {"resnet50": (3, 4, 6), "resnet101": (3, 4, 23)}
+
+
+def _resnet(layers):
+    # resnet.py:57-138: Bottleneck, stride on conv2, layer4 dropped; ResNet50 [3,4,6], ResNet101 [3,4,23] (:178-201)
     enc = ParamNode()
     enc.conv1 = Conv(3, 64, 7, bias=False)
     enc.bn1 = FrozenBN(64)
     inpl = 64
-    for li, (planes, nblk, stride) in enumerate(((64, 3, 1), (128, 4, 2), (256, 6, 2)), start=1):
+    for li, (planes, nblk, stride) in enumerate(zip((64, 128, 256), layers, (1, 2, 2)), start=1):
         blocks = []
         for bi in range(nblk):
             b = ParamNode()
@@ -98,6 +101,50 @@ def _resnet50():
         if isinstance(m, Conv):
             n = m.weight.shape[2] * m.weight.shape[3] * m.weight.shape[0]
             nn.init.normal_(m.weight, 0, math.sqrt(2.0 / n))  # resnet.py:160-163
+    return enc
+
+
+# resnest/resnest.py:51-68 with encoders/__init__.py:28-31 (dilation=2): radix 2, cardinality 1, bottleneck_width 64, deep stem
+# of width 64, avg_down, avd (not first); layers [3, 4, 23] with strides 1, 2, 2 and no dilated conv; layer4 is never built
+RESNEST101_LAYERS = (3, 4, 23)
+
+
+def _resnest101():
+    """Parameter tree of resnest101 with the reference's names (resnest/resnet.py:37-166, 191-357, splat.py:15-78):
+    conv1.{0,1,3,4,6} deep stem + bn1, layer<i>.<j>.{conv1, bn1, conv2.{conv, bn0, fc1, bn1, fc2}, conv3, bn3,
+    downsample.{1,2}} (downsample.0 is the parameter-free AvgPool2d)."""
+    enc = ParamNode()
+    sw = 64
+    enc.conv1 = _seq([Conv(3, sw, 3, bias=False), FrozenBN(sw), ParamNode(), Conv(sw, sw, 3, bias=False), FrozenBN(sw),
+                      ParamNode(), Conv(sw, 2 * sw, 3, bias=False)])
+    enc.bn1 = FrozenBN(2 * sw)
+    inpl = 2 * sw
+    for li, (planes, nblk) in enumerate(zip((64, 128, 256), RESNEST101_LAYERS), start=1):
+        gw = planes                                   # group width: planes * bottleneck_width / 64 * cardinality
+        blocks = []
+        for bi in range(nblk):
+            b = ParamNode()
+            b.conv1 = Conv(inpl, gw, 1, bias=False)
+            b.bn1 = FrozenBN(gw)
+            sp = ParamNode()                          # SplAtConv2d, radix 2: inter_channels = max(gw * 2 // 4, 32)
+            inter = max(gw * 2 // 4, 32)
+            sp.conv = Conv(gw, 2 * gw, 3, bias=False, groups=2)
+            sp.bn0 = FrozenBN(2 * gw)
+            sp.fc1 = Conv(gw, inter, 1)
+            sp.bn1 = FrozenBN(inter)
+            sp.fc2 = Conv(inter, 2 * gw, 1)
+            b.conv2 = sp
+            b.conv3 = Conv(gw, planes * 4, 1, bias=False)
+            b.bn3 = FrozenBN(planes * 4)
+            if bi == 0:                               # stride 2 (layers 2, 3) or inplanes != planes * 4 (layer 1)
+                b.downsample = _seq([ParamNode(), Conv(inpl, planes * 4, 1, bias=False), FrozenBN(planes * 4)])
+            inpl = planes * 4
+            blocks.append(b)
+        setattr(enc, f"layer{li}", _seq(blocks))
+    for m in enc.modules():
+        if isinstance(m, Conv):
+            n = m.weight.shape[2] * m.weight.shape[3] * m.weight.shape[0]
+            nn.init.normal_(m.weight, 0, math.sqrt(2.0 / n))  # resnest/resnet.py:308-311
     return enc
 
 
@@ -201,13 +248,16 @@ def _swin_base():
 
 
 def build_encoder_params(name):
-    if name == "resnet50":
-        return _resnet50()
+    if name in RESNET_LAYERS:
+        return _resnet(RESNET_LAYERS[name])
+    if name == "resnest101":
+        return _resnest101()
     if name == "mobilenetv2":
         return _mobilenetv2()
     if name == "swin_base":
         return _swin_base()
-    raise NotImplementedError(f"encoder '{name}' has no sm_90a path yet (resnet50, mobilenetv2, swin_base do)")
+    raise NotImplementedError(f"encoder '{name}' has no sm_90a path yet (resnet50, resnet101, resnest101, mobilenetv2, "
+                              "swin_base do)")
 
 
 # ---------------------------------------------------------------- transformer blocks

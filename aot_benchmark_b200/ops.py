@@ -402,6 +402,59 @@ def groupnorm(x, gamma, beta, out, G, act, workspace, stream=None):
     return out
 
 
+def splat_workspace(C, device):
+    n = lib().aotb_splat_workspace_bytes(C)
+    return torch.zeros((n + 7) // 8, dtype=torch.float64, device=device)      # zero: the launch counter lives in it
+
+
+def splat_attention(x, w1, b1, w2, b2, att, workspace, radix=2, stream=None):
+    """ResNeSt split attention of one image: x [1,H,W,radix*C] NHWC (or [HW, radix*C]), w1 [C, inter], b1 [inter],
+    w2 [inter, radix*C], b2 [radix*C] -> att [radix*C] (radix-major)."""
+    _chk(x, w1, b1, w2, b2, att)
+    x2 = x.reshape(-1, x.shape[-1]) if x.dim() == 4 else x
+    HW, ld = x2.shape[0], (_nhwc_ld(x) if x.dim() == 4 else x.stride(0))
+    C, inter = w1.shape
+    if w2.shape != (inter, radix * C) or b1.numel() != inter or b2.numel() != radix * C or att.numel() != radix * C \
+            or x.shape[-1] < radix * C or not (w1.is_contiguous() and w2.is_contiguous() and att.is_contiguous()):
+        raise AotbError("splat_attention: shapes x [.., >= radix*C], w1 [C, inter], w2 [inter, radix*C], att [radix*C]")
+    check(lib().aotb_splat_attention_f32(_p(x), ld, HW, C, radix, _p(w1), _p(b1), inter, _p(w2), _p(b2), _p(att),
+                                         workspace.data_ptr(), _st(stream)), "aotb_splat_attention_f32")
+    return att
+
+
+def splat_combine(x, att, out, radix=2, pool_stride=0, stream=None):
+    """x [1,H,W,radix*C], att [radix*C] -> out [1,Ho,Wo,C] = sum_r att_r * x_r, avg-pooled 3x3 / pool_stride / pad 1 if
+    pool_stride > 0."""
+    _chk(x, att, out)
+    _, H, W, _ = x.shape
+    C = out.shape[3]
+    Ho, Wo = (pool2d_size(H, 3, pool_stride, 1), pool2d_size(W, 3, pool_stride, 1)) if pool_stride else (H, W)
+    if att.numel() != radix * C or x.shape[3] < radix * C or tuple(out.shape[1:3]) != (Ho, Wo):
+        raise AotbError(f"splat_combine: x {tuple(x.shape)}, att {tuple(att.shape)}, out {tuple(out.shape)}")
+    check(lib().aotb_splat_combine_f32(_p(x), _nhwc_ld(x), _p(att), _p(out), _nhwc_ld(out), H, W, C, radix, int(pool_stride),
+                                       _st(stream)), "aotb_splat_combine_f32")
+    return out
+
+
+def pool2d_size(n, k, s, pad=0, ceil_mode=False):
+    """Output extent of nn.AvgPool2d / nn.MaxPool2d (dilation 1) along one axis, PyTorch's rule."""
+    o = (n + 2 * pad - k + (s - 1 if ceil_mode else 0)) // s + 1
+    if ceil_mode and (o - 1) * s >= n + pad:
+        o -= 1
+    return o
+
+
+def avgpool(x, out, k, s, pad=0, ceil_mode=False, count_include_pad=True, stream=None):
+    """nn.AvgPool2d(k, s, pad, ceil_mode, count_include_pad) on x [B,H,W,C] -> out [B,Ho,Wo,C]."""
+    _chk(x, out)
+    B, H, W, C = x.shape
+    if tuple(out.shape) != (B, pool2d_size(H, k, s, pad, ceil_mode), pool2d_size(W, k, s, pad, ceil_mode), C):
+        raise AotbError(f"avgpool: out {tuple(out.shape)} does not match x {tuple(x.shape)} pooled ({k}, {s}, {pad})")
+    check(lib().aotb_avgpool_nhwc_f32(_p(x), _nhwc_ld(x), _p(out), _nhwc_ld(out), B, H, W, C, k, s, pad, 1 if ceil_mode else 0,
+                                      1 if count_include_pad else 0, _st(stream)), "aotb_avgpool_nhwc_f32")
+    return out
+
+
 def attention(Q, K, V, O, H, d_qk, d_v, Tk=None, Tk_dev=None, Mout=None, Lout=None, stream=None):
     """Q [N, H*d_qk], K [>=Tk, H*d_qk], V [>=Tk, H*d_v], O [N, H*d_v]."""
     _chk(Q, K, V, O, Mout, Lout)

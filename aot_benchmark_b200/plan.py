@@ -17,7 +17,7 @@ from types import SimpleNamespace as NS
 
 import torch
 
-from .model import SWIN_BASE, mobilenetv2_plan, swin_relative_position_index
+from .model import RESNEST101_LAYERS, RESNET_LAYERS, SWIN_BASE, mobilenetv2_plan, swin_relative_position_index
 
 
 def _signature(model):
@@ -171,9 +171,9 @@ class Plan:
     def _encoder(self, name):
         self.encoder_name = name
         p = "encoder."
-        if name == "resnet50":
+        if name in RESNET_LAYERS:
             e = NS(stem=self._conv_bn(p + "conv1", p + "bn1", pad_cin_to=4), stages=[])   # image is fed as NHWC4
-            for li, (nblk, stride) in enumerate(((3, 1), (4, 2), (6, 2)), start=1):
+            for li, (nblk, stride) in enumerate(zip(RESNET_LAYERS[name], (1, 2, 2)), start=1):
                 blocks = []
                 for bi in range(nblk):
                     q = f"{p}layer{li}.{bi}."
@@ -200,8 +200,43 @@ class Plan:
             self.enc = e
         elif name == "swin_base":
             self.enc = self._swin(p)
+        elif name == "resnest101":
+            self.enc = self._resnest(p)
         else:
             raise NotImplementedError(f"encoder '{name}' has no sm_90a path")
+
+    def _resnest(self, p):
+        """ResNeSt-101 (resnest/resnet.py:191-357, splat.py:15-115) weights: the deep stem as three 3x3 convs (the first over
+        the NHWC4 image), per bottleneck conv1 / conv3 with bn1 / bn3 folded, the radix-2 grouped 3x3 conv of SplAtConv2d as
+        one [9 * gw/2, gw] weight per group with its slice of bn0 folded (each group is one launch on channel slices), fc1 with
+        bn1 folded as [gw, inter] + bias, fc2 as [inter, 2 gw] + bias, and the avg_down downsample conv with its BN folded."""
+        sd = self.sd
+        e = NS(stem=[self._conv_bn(p + "conv1.0", p + "conv1.1", pad_cin_to=4), self._conv_bn(p + "conv1.3", p + "conv1.4"),
+                     self._conv_bn(p + "conv1.6", p + "bn1")], stages=[])
+        for li, (nblk, stride) in enumerate(zip(RESNEST101_LAYERS, (1, 2, 2)), start=1):
+            blocks = []
+            for bi in range(nblk):
+                q = f"{p}layer{li}.{bi}."
+                s = q + "conv2."
+                b = NS(c1=self._conv_bn(q + "conv1", q + "bn1"), c3=self._conv_bn(q + "conv3", q + "bn3"),
+                       stride=stride if bi == 0 else 1, down=None)
+                scale, shift = self._bn(s + "bn0")
+                w = sd[s + "conv.weight"]                                   # [2 gw, gw / 2, 3, 3], groups = 2
+                gw = w.shape[0] // 2
+                b.gw = gw
+                b.groups = [NS(w=self._reg(self._conv_w(w[g * gw:(g + 1) * gw], scale[g * gw:(g + 1) * gw]), w.shape[1]),
+                               b=self._f(shift[g * gw:(g + 1) * gw].float())) for g in range(2)]
+                s1, t1 = self._bn(s + "bn1")                                 # fc1 (1x1 conv with bias) -> bn1, in float64
+                w1 = sd[s + "fc1.weight"].double().flatten(1) * s1.view(-1, 1)
+                b.fc1_w = self._f(w1.t().float())                           # [gw, inter]
+                b.fc1_b = self._f((sd[s + "fc1.bias"].double() * s1 + t1).float())
+                b.fc2_w = self._f(sd[s + "fc2.weight"].flatten(1).t())      # [inter, 2 gw]
+                b.fc2_b = self._f(sd[s + "fc2.bias"])
+                if (q + "downsample.1.weight") in sd:
+                    b.down = self._conv_bn(q + "downsample.1", q + "downsample.2")
+                blocks.append(b)
+            e.stages.append(blocks)
+        return e
 
     def _swin(self, p):
         """Swin-B (build.py:11-22) weights: every Linear as [in, out] (registered for the tensor-core GEMM), the 4x4/4

@@ -119,6 +119,27 @@ size_t aotb_groupnorm_workspace_bytes(int B, int G);
 int aotb_groupnorm_nhwc_f32(const float* x, int ldx, const float* gamma, const float* beta, float* out, int ldo,
                             int B, int P, int C, int G, int act, void* workspace, void* stream);
 
+/* Split attention of ResNeSt (SplAtConv2d after its grouped conv + bn0 + ReLU, cardinality 1), one image:
+ * networks/encoders/resnest/splat.py:88-105,118-132.  x [HW][ldx] holds `radix` splits of C channels (split r = channels
+ * [r*C, (r+1)*C)); gap = mean over pixels of the sum of the splits, h = ReLU(gap @ w1 + b1) with w1 [C][inter] / b1 [inter] = fc1
+ * with bn1 folded, logits = h @ w2 + b2 with w2 [inter][radix*C] / b2 [radix*C] = fc2, att [radix*C] = softmax over r of
+ * logits[r*C + c] (radix-major, as rSoftMax writes it).  C % 4 == 0, C <= 512, inter <= 512, 2 <= radix <= 4.  The pixel sums are
+ * per-CTA partials in the workspace, added in CTA order by the CTA that finishes last (deterministic).  The workspace
+ * (aotb_splat_workspace_bytes(C) bytes, reusable for any smaller C) must be zero-filled before its first use: it holds the launch
+ * counter, which every launch leaves at zero again (graph replays start from the same state). */
+size_t aotb_splat_workspace_bytes(int C);
+int aotb_splat_attention_f32(const float* x, int ldx, int HW, int C, int radix, const float* w1, const float* b1, int inter,
+                             const float* w2, const float* b2, float* att, void* workspace, void* stream);
+/* out [Ho][Wo][ldo] = sum_r att[r*C + c] * x[r*C + c] (splat.py:107-113), one image x [H][W][ldx].  pool_stride > 0 also applies the
+ * avd pool nn.AvgPool2d(3, pool_stride, padding=1) (padding counted; networks/encoders/resnest/resnet.py:72-73,152-153), so the
+ * full-resolution sum is never written; pool_stride 0: Ho = H, Wo = W. */
+int aotb_splat_combine_f32(const float* x, int ldx, const float* att, float* out, int ldo, int H, int W, int C, int radix,
+                           int pool_stride, void* stream);
+/* nn.AvgPool2d(k, s, pad, ceil_mode, count_include_pad) in NHWC, in [B][H][W][ldin] -> out [B][Ho][Wo][ldo] with PyTorch's
+ * output extent and divisor rules: networks/encoders/resnest/resnet.py:330-342 (avg_down). */
+int aotb_avgpool_nhwc_f32(const float* in, int ldin, float* out, int ldo, int B, int H, int W, int C, int k, int s, int pad,
+                          int ceil_mode, int count_include_pad, void* stream);
+
 /* softmax((Q/T) K^T) V per head, scores never materialised (fp32 reference-precision path).
  * networks/layers/attention.py:82-117 (MultiheadAttention) and :672-704 (GatedPropagation).
  * Tk_dev (optional) is a device int holding the live key count.  With Mout/Lout the kernel writes
