@@ -63,6 +63,13 @@ constexpr int GN_CHUNKS = 64;
 
 // `chunks` (a multiple of 8, <= GN_CHUNKS) pixel ranges per (b, g): enough blocks to fill the GPU on the large decoder maps, few
 // enough on the 31 x 54 token maps that a block has more than one load per thread (2 048 blocks of 208 float4 took 9.8 us).
+//
+// The sums are taken about a shift K = x[b][0][g*Cg], the first element of the group: S = sum(v - K), Q = sum((v - K)^2), and
+// the finaliser forms mean = K + S/n, var = Q/n - (S/n)^2.  The raw sums sum(v), sum(v^2) cancel catastrophically in
+// E[v^2] - mean^2 once |mean| is large next to the standard deviation (on the FFN shape at mean/std = 1000, gamma = 1, the
+// raw-sum form was off by 4.8e-2 on an H100, the shifted one by 4.1e-5); about K the cancellation is only that of
+// (K - mean)^2, a few variances.  Every block reads the same K, so the result does not
+// depend on the launch.
 __global__ void groupnorm_stats_kernel(const float* __restrict__ x, int ldx, int P, int G, int Cg,
                                        double* __restrict__ partial, float* __restrict__ stat, unsigned* __restrict__ counter,
                                        float eps) {
@@ -71,14 +78,16 @@ __global__ void groupnorm_stats_kernel(const float* __restrict__ x, int ldx, int
     const int per = (P + chunks - 1) / chunks;
     const int p0 = chunk * per, p1 = min(P, p0 + per);
     const float* xb = x + (size_t)b * P * ldx + (size_t)g * Cg;
+    const float K = xb[0];
     const int Cg4 = Cg >> 2;
     float s = 0.f, q = 0.f;
     const int n = (p1 > p0 ? (p1 - p0) : 0) * Cg4;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const int p = p0 + i / Cg4, c = (i % Cg4) * 4;
-        float4 v = *reinterpret_cast<const float4*>(xb + (size_t)p * ldx + c);
-        s += (v.x + v.y) + (v.z + v.w);
-        q += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
+        const float4 v = *reinterpret_cast<const float4*>(xb + (size_t)p * ldx + c);
+        const float a = v.x - K, bb = v.y - K, cc = v.z - K, d = v.w - K;
+        s += (a + bb) + (cc + d);
+        q += (a * a + bb * bb) + (cc * cc + d * d);
     }
     __shared__ double sh[2][8];
     __shared__ unsigned last;
@@ -115,11 +124,13 @@ __global__ void groupnorm_stats_kernel(const float* __restrict__ x, int ldx, int
             qq += __shfl_xor_sync(0xffffffffu, qq, o);
         }
         if (bg < BG && sub == 0) {
+            // the shift of this (b, g), as its stats blocks read it: x is not written before the apply kernel runs
+            const double shift = x[(size_t)(bg / G) * P * ldx + (size_t)(bg % G) * Cg];
             const double nn = (double)P * Cg;
-            const double mean = ss / nn;
-            double var = qq / nn - mean * mean;
+            const double dm = ss / nn;
+            double var = qq / nn - dm * dm;
             if (var < 0) var = 0;
-            stat[2 * bg] = (float)mean;
+            stat[2 * bg] = (float)(shift + dm);
             stat[2 * bg + 1] = (float)(1.0 / sqrt(var + (double)eps));
         }
     }
