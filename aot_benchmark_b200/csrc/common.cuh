@@ -88,7 +88,10 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // activation codes shared by several entry points
-enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_SILU = 3, ACT_RELU6 = 4 };
+enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_SILU = 3, ACT_RELU6 = 4, ACT_HSWISH = 5 };
+
+// h_sigmoid(v) = relu6(v + 3) / 6 with a true division, as networks/encoders/mobilenetv3.py:33-39 computes it
+__device__ __forceinline__ float hsigmoid(float v) { return fminf(fmaxf(v + 3.f, 0.f), 6.f) / 6.f; }
 
 __device__ __forceinline__ float apply_act(float v, int act) {
     switch (act) {
@@ -98,6 +101,18 @@ __device__ __forceinline__ float apply_act(float v, int act) {
         case ACT_RELU6: return fminf(fmaxf(v, 0.f), 6.f);
         default: return v;
     }
+}
+
+// h_swish = v * h_sigmoid(v) (mobilenetv3.py:42-48) stays out of apply_act, so every kernel that existed before it compiles
+// exactly as before.  The kernels MobileNetV3 runs take it as a template flag (fp32 conv finish, depthwise conv: HS selects the
+// instantiation, so the existing ones are unchanged) or as a runtime code (gate scale, apply_act_hs); the tensor-core conv, the
+// conv chain and GroupNorm reject ACT_HSWISH at their entry points.
+template <bool HS>
+__device__ __forceinline__ float apply_act_or_hswish(float v, int act) {
+    return HS ? v * hsigmoid(v) : apply_act(v, act);
+}
+__device__ __forceinline__ float apply_act_hs(float v, int act) {
+    return act == ACT_HSWISH ? v * hsigmoid(v) : apply_act(v, act);
 }
 
 }  // namespace aotb

@@ -288,6 +288,8 @@ int plan_chain(const aotb_chain_layer* ls, int n, ChainPlan& P) {
         AOTB_REQUIRE(l.in && l.wh && l.wl && l.out, "aotb_conv_chain: layer %d: null pointer", i);
         AOTB_REQUIRE(l.Cin % 64 == 0 && l.Cout % 64 == 0, "aotb_conv_chain: layer %d: Cin and Cout must be multiples of 64", i);
         AOTB_REQUIRE(l.ldin % 4 == 0 && l.ldout % 4 == 0 && (!l.res || l.ldres % 4 == 0), "aotb_conv_chain: layer %d: strides", i);
+        AOTB_REQUIRE(l.act >= ACT_NONE && l.act <= ACT_RELU6, "aotb_conv_chain: layer %d: activation %d not supported (0-4)", i,
+                     l.act);
         AOTB_REQUIRE(l.in_layer < i && l.res_layer < i, "aotb_conv_chain: layer %d: producers must come earlier in the chain", i);
         tc::ChainLayer d{};
         d.in = l.in; d.bias = l.bias; d.wscale = l.wscale; d.res = l.res; d.out = l.out;

@@ -32,7 +32,7 @@ struct ConvArgs {
     int ovec;  // out base 16B-aligned and ldout % 4 == 0
 };
 
-template <int BM, int BN, int TM, int TN, bool AVEC, bool BVEC>
+template <int BM, int BN, int TM, int TN, bool AVEC, bool BVEC, bool HS = false>
 __global__ void __launch_bounds__(256) conv_igemm_kernel(const ConvArgs p) {
     pdl_sync();
     constexpr int BK = 16;
@@ -246,7 +246,7 @@ __global__ void __launch_bounds__(256) conv_igemm_kernel(const ConvArgs p) {
                 if (nn < p.Cout) {
                     if (p.bias) x += __ldg(p.bias + nn);
                     if (rrow) x += rrow[nn];
-                    x = apply_act(x, p.act);
+                    x = apply_act_or_hswish<HS>(x, p.act);
                 }
                 v[j] = x;
             }
@@ -264,7 +264,10 @@ __global__ void __launch_bounds__(256) conv_igemm_kernel(const ConvArgs p) {
 template <int BM, int BN, int TM, int TN, bool AVEC, bool BVEC>
 static void launch_conv(const ConvArgs& a, cudaStream_t st) {
     dim3 grid(cdiv(a.M, BM), cdiv(a.Cout, BN));
-    launch(conv_igemm_kernel<BM, BN, TM, TN, AVEC, BVEC>, dim3(grid), dim3(256), 0, st, a);
+    if (a.act == ACT_HSWISH)
+        launch(conv_igemm_kernel<BM, BN, TM, TN, AVEC, BVEC, true>, dim3(grid), dim3(256), 0, st, a);
+    else
+        launch(conv_igemm_kernel<BM, BN, TM, TN, AVEC, BVEC>, dim3(grid), dim3(256), 0, st, a);
 }
 
 int conv2d_dispatch(const ConvArgs& a, cudaStream_t st) {

@@ -339,6 +339,7 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
                                    void* stream) {
     AOTB_REQUIRE(in && wh && wl && out, "aotb_conv2d_nhwc_tc: null pointer");
     AOTB_REQUIRE(Cin % 4 == 0 && Cout % 64 == 0, "aotb_conv2d_nhwc_tc: Cin must be a multiple of 4, Cout of 64");
+    AOTB_REQUIRE(act >= aotb::ACT_NONE && act <= aotb::ACT_RELU6, "aotb_conv2d_nhwc_tc: activation %d not supported (0-4)", act);
     AOTB_REQUIRE(ldin % 4 == 0 && ldout % 4 == 0 && (!res || ldres % 4 == 0) && ((uintptr_t)in % 16 == 0) &&
                      ((uintptr_t)out % 16 == 0) && (!res || (uintptr_t)res % 16 == 0) && (!bias || (uintptr_t)bias % 16 == 0) &&
                      (!wscale || (uintptr_t)wscale % 16 == 0),

@@ -67,6 +67,7 @@ __global__ void maxpool3x3s2_kernel(const float4* __restrict__ in, float4* __res
 
 // ---------------------------------------------------------------- depthwise conv (NHWC, C%4==0)
 // w layout [KH*KW][C]; optional per-channel bias; optional activation.
+template <bool HS = false>
 __global__ void dwconv_kernel(const float* __restrict__ in, const float* __restrict__ w,
                               const float* __restrict__ bias, float* __restrict__ out, int B, int H, int W, int C,
                               int ldin, int ldout, int Ho, int Wo, int KH, int KW, int stride, int pad, int dil,
@@ -93,8 +94,8 @@ __global__ void dwconv_kernel(const float* __restrict__ in, const float* __restr
                 acc.z = fmaf(v.z, ww.z, acc.z); acc.w = fmaf(v.w, ww.w, acc.w);
             }
         }
-        acc.x = apply_act(acc.x, act); acc.y = apply_act(acc.y, act);
-        acc.z = apply_act(acc.z, act); acc.w = apply_act(acc.w, act);
+        acc.x = apply_act_or_hswish<HS>(acc.x, act); acc.y = apply_act_or_hswish<HS>(acc.y, act);
+        acc.z = apply_act_or_hswish<HS>(acc.z, act); acc.w = apply_act_or_hswish<HS>(acc.w, act);
         *reinterpret_cast<float4*>(out + (((size_t)b * Ho + oy) * Wo + ox) * ldout + c) = acc;
     }
 }
@@ -102,7 +103,7 @@ __global__ void dwconv_kernel(const float* __restrict__ in, const float* __restr
 // Stride-1, dilation-1 K x K depthwise conv (the 5x5 of the LSTT / GPM feed-forward): one thread = 4 neighbouring
 // output pixels x 4 channels.  The K+3 inputs of a filter row and its K weights are loaded once and shared by the 4
 // outputs (K*(K+3) + K*K loads per 4*K*K taps instead of 2 per tap -- the generic kernel above is L1-bandwidth bound).
-template <int K>
+template <int K, bool HS = false>
 __global__ void dwconv_row4_kernel(const float* __restrict__ in, const float* __restrict__ w,
                                    const float* __restrict__ bias, float* __restrict__ out, int B, int H, int W, int C,
                                    int ldin, int ldout, int pad, int act) {
@@ -144,7 +145,8 @@ __global__ void dwconv_row4_kernel(const float* __restrict__ in, const float* __
         for (int o = 0; o < 4; ++o) {
             if (ox0 + o >= Wo) break;
             float4 r = acc[o];
-            r.x = apply_act(r.x, act); r.y = apply_act(r.y, act); r.z = apply_act(r.z, act); r.w = apply_act(r.w, act);
+            r.x = apply_act_or_hswish<HS>(r.x, act); r.y = apply_act_or_hswish<HS>(r.y, act);
+            r.z = apply_act_or_hswish<HS>(r.z, act); r.w = apply_act_or_hswish<HS>(r.w, act);
             *reinterpret_cast<float4*>(out + (((size_t)b * Ho + oy) * Wo + ox0 + o) * ldout + c) = r;
         }
     }
@@ -274,12 +276,12 @@ extern "C" int aotb_dwconv_nhwc_f32(const float* in, const float* w, const float
     const int Wo = (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
     if (KH == 5 && KW == 5 && stride == 1 && dil == 1) {
         const size_t tot4 = (size_t)B * Ho * ((Wo + 3) / 4) * (C / 4);
-        launch(dwconv_row4_kernel<5>, dim3(grid_for(tot4, 128)), dim3(128), 0, (cudaStream_t)stream, in, w, bias, out, B, H, W,
+        launch(act == ACT_HSWISH ? dwconv_row4_kernel<5, true> : dwconv_row4_kernel<5>, dim3(grid_for(tot4, 128)), dim3(128), 0, (cudaStream_t)stream, in, w, bias, out, B, H, W,
                C, ldin, ldout, pad, act);
         return check_launch("aotb_dwconv_nhwc_f32");
     }
     const size_t total = (size_t)B * Ho * Wo * (C / 4);
-    launch(dwconv_kernel, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, in, w, bias, out, B, H, W, C, ldin, ldout,
+    launch(act == ACT_HSWISH ? dwconv_kernel<true> : dwconv_kernel<>, dim3(grid_for(total, 256)), dim3(256), 0, (cudaStream_t)stream, in, w, bias, out, B, H, W, C, ldin, ldout,
                                                                          Ho, Wo, KH, KW, stride, pad, dil, act);
     return check_launch("aotb_dwconv_nhwc_f32");
 }

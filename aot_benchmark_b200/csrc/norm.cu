@@ -195,6 +195,7 @@ extern "C" int aotb_groupnorm_nhwc_f32(const float* x, int ldx, const float* gam
     AOTB_REQUIRE(x && gamma && beta && out && workspace, "aotb_groupnorm_nhwc_f32: null pointer");
     AOTB_REQUIRE(G > 0 && C % G == 0 && (C / G) % 4 == 0 && ldx % 4 == 0 && ldo % 4 == 0 && G <= 1024,
                  "aotb_groupnorm_nhwc_f32: unsupported channel/group configuration");
+    AOTB_REQUIRE(act >= ACT_NONE && act <= ACT_RELU6, "aotb_groupnorm_nhwc_f32: activation %d not supported (0-4)", act);
     const int Cg = C / G;
     cudaStream_t st = (cudaStream_t)stream;
     unsigned* counter = (unsigned*)workspace;

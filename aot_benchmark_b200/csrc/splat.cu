@@ -1,14 +1,15 @@
-// Split-attention (ResNeSt) and average pooling, NHWC fp32.
+// Split-attention (ResNeSt), squeeze-excite (MobileNetV3) and average pooling, NHWC fp32.
 //
 // Reference sites: networks/encoders/resnest/splat.py:88-115 (SplAtConv2d.forward after its grouped conv + bn0 + ReLU:
 // gap, fc1 + bn1 + ReLU, fc2, rSoftMax :118-132, the attention-weighted sum of the radix splits),
 // networks/encoders/resnest/resnet.py:72-73,152-153 (avd AvgPool2d(3, stride, padding=1) after conv2) and :330-342
-// (avg_down AvgPool2d(stride, stride, ceil_mode=True, count_include_pad=False) in front of the downsample conv).
+// (avg_down AvgPool2d(stride, stride, ceil_mode=True, count_include_pad=False) in front of the downsample conv);
+// networks/encoders/mobilenetv3.py:51-65 (SELayer: mean over the map, fc1 + ReLU, fc2 + h_sigmoid, x * gate).
 //
 // The pixel reduction of the split attention spans many CTAs.  Each CTA writes the per-channel sum of its fixed pixel range
 // to its own slot of the workspace (double), and the CTA that takes the last ticket of the launch counter adds the slots in
-// CTA order, runs the two small GEMVs and the radix softmax, and resets the counter: the result does not depend on CTA
-// scheduling, and every launch (or graph replay) starts from a zero counter.
+// CTA order, runs the two small GEMVs and the final gate (radix softmax or h_sigmoid), and resets the counter: the result
+// does not depend on CTA scheduling, and every launch (or graph replay) starts from a zero counter.
 #include "common.cuh"
 #include <cstdint>
 
@@ -16,12 +17,16 @@ namespace aotb {
 
 constexpr int SPLAT_THREADS = 256;
 constexpr int SPLAT_MAX_CTAS = 264;          // 2 per SM
-constexpr int SPLAT_MAX_C = 512;
+constexpr int SPLAT_MAX_C = 1024;         // one float4 channel group per thread: C / 4 <= SPLAT_THREADS
 constexpr int SPLAT_MAX_RADIX = 4;
 constexpr size_t SPLAT_HDR = 256;            // launch counter
 
+enum Gate { GATE_RSOFTMAX = 0, GATE_HSIGMOID = 1 };
+
 // x [HW][ldx] holds radix splits of C channels: split r = channels [r*C, (r+1)*C).
 // w1 [C][inter] (fc1 with bn1 folded), b1 [inter], w2 [inter][radix*C] (fc2), b2 [radix*C] -> att [radix*C] (radix-major).
+// GATE_RSOFTMAX: softmax across the radix (ResNeSt); GATE_HSIGMOID: radix 1, att = h_sigmoid(logit) (squeeze-excite).
+template <int GATE>
 __global__ void __launch_bounds__(SPLAT_THREADS)
 splat_attention_kernel(const float* __restrict__ x, int ldx, int HW, int C, int radix, const float* __restrict__ w1,
                        const float* __restrict__ b1, int inter, const float* __restrict__ w2, const float* __restrict__ b2,
@@ -85,6 +90,11 @@ splat_attention_kernel(const float* __restrict__ x, int ldx, int HW, int C, int 
         logit[k] = a;
     }
     __syncthreads();
+    if (GATE == GATE_HSIGMOID) {
+        for (int c = tid; c < C; c += SPLAT_THREADS) att[c] = hsigmoid(logit[c]);
+        if (tid == 0) *counter = 0u;
+        return;
+    }
     // rSoftMax: softmax across the radix for every channel (cardinality 1), written radix-major
     for (int c = tid; c < C; c += SPLAT_THREADS) {
         float m = logit[c];
@@ -112,11 +122,12 @@ __device__ __forceinline__ PoolWin pool_window(int oy, int ox, int H, int W, int
     return PoolWin{y0, y1, x0, x1, (float)div};
 }
 
-// out [Ho][Wo][ldo] (C channels) = sum_r att[r*C + c] * x[r*C + c], optionally average-pooled 3x3 / stride / pad 1 with padding
-// counted (pool_stride 0: no pool, Ho = H, Wo = W).  The radix is a template argument so the weights stay in registers.
+// out [Ho][Wo][ldo] (C channels) = act(sum_r att[r*C + c] * x[r*C + c]), optionally average-pooled 3x3 / stride / pad 1 with
+// padding counted before the activation (pool_stride 0: no pool, Ho = H, Wo = W).  The radix is a template argument so the
+// weights stay in registers.  With radix 1 the sum is the single rounded product att * x, as the reference's x * y computes it.
 template <int RADIX>
 __global__ void splat_combine_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ att, float* __restrict__ out,
-                                     int ldo, int H, int W, int C, int pool_stride, int Ho, int Wo) {
+                                     int ldo, int H, int W, int C, int pool_stride, int Ho, int Wo, int act) {
     pdl_sync();
     const int C4 = C >> 2;
     const size_t total = (size_t)Ho * Wo * C4;
@@ -151,6 +162,7 @@ __global__ void splat_combine_kernel(const float* __restrict__ x, int ldx, const
                 }
             o.x /= pw.div; o.y /= pw.div; o.z /= pw.div; o.w /= pw.div;
         }
+        o.x = apply_act_hs(o.x, act); o.y = apply_act_hs(o.y, act); o.z = apply_act_hs(o.z, act); o.w = apply_act_hs(o.w, act);
         *reinterpret_cast<float4*>(out + ((size_t)oy * Wo + ox) * ldo + c) = o;
     }
 }
@@ -213,7 +225,7 @@ extern "C" int aotb_splat_attention_f32(const float* x, int ldx, int HW, int C, 
     ctas = ctas > SPLAT_MAX_CTAS ? SPLAT_MAX_CTAS : ctas;
     unsigned* counter = (unsigned*)workspace;
     double* partial = (double*)((uint8_t*)workspace + SPLAT_HDR);
-    launch(splat_attention_kernel, dim3(ctas), dim3(SPLAT_THREADS), 0, (cudaStream_t)stream, x, ldx, HW, C, radix, w1, b1,
+    launch(splat_attention_kernel<GATE_RSOFTMAX>, dim3(ctas), dim3(SPLAT_THREADS), 0, (cudaStream_t)stream, x, ldx, HW, C, radix, w1, b1,
            inter, w2, b2, att, partial, counter);
     return check_launch("aotb_splat_attention_f32");
 }
@@ -233,8 +245,38 @@ extern "C" int aotb_splat_combine_f32(const float* x, int ldx, const float* att,
     auto kernel = radix == 1 ? splat_combine_kernel<1> : radix == 2 ? splat_combine_kernel<2>
                 : radix == 3 ? splat_combine_kernel<3> : splat_combine_kernel<4>;
     launch(kernel, dim3(grid_for(total)), dim3(256), 0, (cudaStream_t)stream, x, ldx, att, out, ldo, H, W, C, pool_stride, Ho,
-           Wo);
+           Wo, (int)ACT_NONE);
     return check_launch("aotb_splat_combine_f32");
+}
+
+extern "C" int aotb_se_gate_f32(const float* x, int ldx, int HW, int C, const float* w1, const float* b1, int inter,
+                                const float* w2, const float* b2, float* gate, void* workspace, void* stream) {
+    AOTB_REQUIRE(x && w1 && b1 && w2 && b2 && gate && workspace, "aotb_se_gate_f32: null pointer");
+    AOTB_REQUIRE(HW > 0 && C > 0 && C % 4 == 0 && C <= SPLAT_MAX_C && inter > 0 && inter <= SPLAT_MAX_C && ldx >= C,
+                 "aotb_se_gate_f32: need HW > 0, C %% 4 == 0, C and inter <= %d, ldx >= C", SPLAT_MAX_C);
+    AOTB_REQUIRE(ldx % 4 == 0 && (uintptr_t)x % 16 == 0, "aotb_se_gate_f32: x needs 16-byte aligned rows");
+    const int rows = (SPLAT_THREADS / (C / 4)) * 8;
+    int ctas = cdiv(HW, rows);
+    ctas = ctas > SPLAT_MAX_CTAS ? SPLAT_MAX_CTAS : ctas;
+    unsigned* counter = (unsigned*)workspace;
+    double* partial = (double*)((uint8_t*)workspace + SPLAT_HDR);
+    launch(splat_attention_kernel<GATE_HSIGMOID>, dim3(ctas), dim3(SPLAT_THREADS), 0, (cudaStream_t)stream, x, ldx, HW, C, 1,
+           w1, b1, inter, w2, b2, gate, partial, counter);
+    return check_launch("aotb_se_gate_f32");
+}
+
+extern "C" int aotb_gate_scale_f32(const float* x, int ldx, const float* gate, float* out, int ldo, int HW, int C, int act,
+                                   void* stream) {
+    AOTB_REQUIRE(x && gate && out, "aotb_gate_scale_f32: null pointer");
+    AOTB_REQUIRE(HW > 0 && C > 0 && C % 4 == 0 && ldx >= C && ldo >= C && act >= ACT_NONE && act <= ACT_HSWISH,
+                 "aotb_gate_scale_f32: bad shape or activation");
+    AOTB_REQUIRE(ldx % 4 == 0 && ldo % 4 == 0 && (uintptr_t)x % 16 == 0 && (uintptr_t)out % 16 == 0 &&
+                     (uintptr_t)gate % 16 == 0,
+                 "aotb_gate_scale_f32: 16-byte alignment required");
+    const size_t total = (size_t)HW * (C / 4);
+    launch(splat_combine_kernel<1>, dim3(grid_for(total)), dim3(256), 0, (cudaStream_t)stream, x, ldx, gate, out, ldo, 1, HW, C,
+           0, 1, HW, act);
+    return check_launch("aotb_gate_scale_f32");
 }
 
 extern "C" int aotb_avgpool_nhwc_f32(const float* in, int ldin, float* out, int ldo, int B, int H, int W, int C, int k,

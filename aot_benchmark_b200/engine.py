@@ -25,6 +25,7 @@ from . import ops
 from .plan import get_plan
 
 A_NONE, A_RELU, A_GELU, A_SILU, A_RELU6 = ops.ACT_NONE, ops.ACT_RELU, ops.ACT_GELU, ops.ACT_SILU, ops.ACT_RELU6
+A_HSWISH = ops.ACT_HSWISH
 
 # bench.py hook: when set to a list, every long-term attention launch appends
 # (start_event, end_event, algorithmic_flops) so the roofline is measured live, per launch.
@@ -225,10 +226,12 @@ class _Encoder:
             return self._resnet_chain(x, st)
         if P.encoder_name in ("resnet50", "resnet101"):
             feats = self._resnet(x, st)
-        elif P.encoder_name == "resnest101":
+        elif P.encoder_name in ("resnest50", "resnest101"):
             feats = self._resnest(x, st)
         elif P.encoder_name == "swin_base":
             feats = self._swin(x, st)
+        elif P.encoder_name == "mobilenetv3":
+            feats = self._mobilenetv3(x, st)
         else:
             feats = self._mobilenet(x, st)
         f16 = feats[-1]
@@ -265,7 +268,7 @@ class _Encoder:
         return feats
 
     def _resnest(self, x, st):
-        """ResNeSt-101 (resnest/resnet.py:418-435): deep stem, max-pool, then per bottleneck conv1, the radix-2 grouped 3x3 conv
+        """ResNeSt-50 / ResNeSt-101 (resnest/resnet.py:418-435): deep stem, max-pool, then per bottleneck conv1, the radix-2 grouped 3x3 conv
         as one tensor-core launch per group on channel slices (group g reads channels [g gw/2, (g+1) gw/2) of t1 and writes
         [g gw, (g+1) gw) of t2), the split attention (pixel reduction + fc1 / fc2 / radix softmax in one launch), the
         attention-weighted sum of the two splits (with the avd pool fused in the strided first blocks), the avg_down
@@ -397,6 +400,49 @@ class _Encoder:
                 x = self._buf(f"s{si + 1}x", (H2 * W2, 2 * C))
                 ops.linear(mln, stg.down.w, stg.down.b, x, stream=st)
                 H, W, C = H2, W2, 2 * C
+        return feats
+
+    def _mobilenetv3(self, x, st):
+        """MobileNetV3-Large (mobilenetv3.py:135-215): the 3x3/2 stem with h_swish, then per InvertedResidual the expand conv
+        with the block's activation, the depthwise conv (with the activation when the block has no SE), for SE blocks the gate
+        (pixel mean, fc1 + ReLU, fc2 + h_sigmoid in one launch) and gate * x with the activation (the reference applies the
+        SE before the activation, :127-129), then the pw-linear conv with the residual fused.  Taps after blocks 3, 6 and 12;
+        the last tap is the 1x1 960 conv with h_swish."""
+        e = self.plan.enc
+        H, W = x.shape[1], x.shape[2]
+        h, w = self._osz(H, 3, 2, 1), self._osz(W, 3, 2, 1)
+        cur = self._buf("stem", (1, h, w, e.stem.cout))
+        ops.conv2d(x, e.stem.w, e.stem.b, cur, KH=3, KW=3, stride=2, pad=1, act=A_HSWISH, stream=st)
+        ws = self.bufs.get("se_ws")            # zero-filled once (launch counter), kept for the encoder's lifetime
+        if ws is None:
+            ws = self.bufs["se_ws"] = ops.splat_workspace(max(b.dw.cout for b in e.blocks if b.se is not None), self.dev)
+        feats = []
+        for i, b in enumerate(e.blocks):
+            act = A_HSWISH if b.hs else A_RELU
+            y = cur
+            if b.expand is not None:
+                t = self._buf(f"b{i}e", (1, h, w, b.expand.cout))
+                ops.conv2d(y, b.expand.w, b.expand.b, t, act=act, stream=st)
+                y = t
+            pad = (b.k - 1) // 2 * b.dil                                       # mobilenetv3.py:119-125
+            ho, wo = self._osz(h, b.k, b.stride, pad, b.dil), self._osz(w, b.k, b.stride, pad, b.dil)
+            t = self._buf(f"b{i}d", (1, ho, wo, b.dw.cout))
+            ops.dwconv(y, b.dw.w, b.dw.b, t, K=b.k, stride=b.stride, pad=pad, dil=b.dil,
+                       act=A_NONE if b.se is not None else act, stream=st)
+            if b.se is not None:
+                gate = self._buf(f"b{i}gate", (b.dw.cout,))
+                ops.se_gate(t, b.se.w1, b.se.b1, b.se.w2, b.se.b2, gate, ws, stream=st)
+                g = self._buf(f"b{i}g", (1, ho, wo, b.dw.cout))
+                ops.gate_scale(t, gate, g, act=act, stream=st)
+                t = g
+            o = self._buf(f"b{i}o", (1, ho, wo, b.pw.cout))
+            ops.conv2d(t, b.pw.w, b.pw.b, o, res=cur if b.res else None, stream=st)
+            cur, h, w = o, ho, wo
+            if b.tap:
+                feats.append(cur)
+        last = self._buf("last", (1, h, w, e.last.cout))
+        ops.conv2d(cur, e.last.w, e.last.b, last, act=A_HSWISH, stream=st)
+        feats.append(last)
         return feats
 
     def _mobilenet(self, x, st):

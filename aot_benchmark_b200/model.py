@@ -104,22 +104,21 @@ def _resnet(layers):
     return enc
 
 
-# resnest/resnest.py:51-68 with encoders/__init__.py:28-31 (dilation=2): radix 2, cardinality 1, bottleneck_width 64, deep stem
-# of width 64, avg_down, avd (not first); layers [3, 4, 23] with strides 1, 2, 2 and no dilated conv; layer4 is never built
-RESNEST101_LAYERS = (3, 4, 23)
+# resnest/resnest.py:32-68 with encoders/__init__.py:24-31 (dilation=2): radix 2, cardinality 1, bottleneck_width 64, deep
+# stem, avg_down, avd (not first); strides 1, 2, 2 and no dilated conv; layer4 is never built.  name: (layers, stem_width)
+RESNEST = {"resnest50": ((3, 4, 6), 32), "resnest101": ((3, 4, 23), 64)}
 
 
-def _resnest101():
-    """Parameter tree of resnest101 with the reference's names (resnest/resnet.py:37-166, 191-357, splat.py:15-78):
-    conv1.{0,1,3,4,6} deep stem + bn1, layer<i>.<j>.{conv1, bn1, conv2.{conv, bn0, fc1, bn1, fc2}, conv3, bn3,
-    downsample.{1,2}} (downsample.0 is the parameter-free AvgPool2d)."""
+def _resnest(layers, sw):
+    """Parameter tree of resnest50 / resnest101 with the reference's names (resnest/resnet.py:37-166, 191-357,
+    splat.py:15-78): conv1.{0,1,3,4,6} deep stem (3 -> sw -> sw -> 2 sw) + bn1, layer<i>.<j>.{conv1, bn1, conv2.{conv, bn0,
+    fc1, bn1, fc2}, conv3, bn3, downsample.{1,2}} (downsample.0 is the parameter-free AvgPool2d)."""
     enc = ParamNode()
-    sw = 64
     enc.conv1 = _seq([Conv(3, sw, 3, bias=False), FrozenBN(sw), ParamNode(), Conv(sw, sw, 3, bias=False), FrozenBN(sw),
                       ParamNode(), Conv(sw, 2 * sw, 3, bias=False)])
     enc.bn1 = FrozenBN(2 * sw)
     inpl = 2 * sw
-    for li, (planes, nblk) in enumerate(zip((64, 128, 256), RESNEST101_LAYERS), start=1):
+    for li, (planes, nblk) in enumerate(zip((64, 128, 256), layers), start=1):
         gw = planes                                   # group width: planes * bottleneck_width / 64 * cardinality
         blocks = []
         for bi in range(nblk):
@@ -247,17 +246,95 @@ def _swin_base():
     return enc
 
 
+def _make_divisible(v, divisor=8):
+    # mobilenetv3.py:13-30
+    new_v = max(divisor, int(v + divisor / 2) // divisor * divisor)
+    return new_v + divisor if new_v < 0.9 * v else new_v
+
+
+# mobilenetv3.py:152-169: k, t, c, SE, HS, s
+_MBV3_CFGS = [[3, 1, 16, 0, 0, 1], [3, 4, 24, 0, 0, 2], [3, 3, 24, 0, 0, 1], [5, 3, 40, 1, 0, 2], [5, 3, 40, 1, 0, 1],
+              [5, 3, 40, 1, 0, 1], [3, 6, 80, 0, 1, 2], [3, 2.5, 80, 0, 1, 1], [3, 2.3, 80, 0, 1, 1], [3, 2.3, 80, 0, 1, 1],
+              [3, 6, 112, 1, 1, 1], [3, 6, 112, 1, 1, 1], [5, 6, 160, 1, 1, 2], [5, 6, 160, 1, 1, 1], [5, 6, 160, 1, 1, 1]]
+
+
+def mobilenetv3_plan(output_stride=16):
+    """(inp, hidden, oup, k, stride, dilation, se, hs) per InvertedResidual of MobileNetV3Large (mobilenetv3.py:172-192,
+    width_mult 1), and the width of the last 1x1 conv (:195)."""
+    plan, inp, cur, rate = [], _make_divisible(16), 2, 1
+    for k, t, c, se, hs, s in _MBV3_CFGS:
+        if cur == output_stride:
+            dil = rate
+            rate *= s
+            s = 1
+        else:
+            dil = 1
+            cur *= s
+        oup, hid = _make_divisible(c), _make_divisible(inp * t)
+        plan.append((inp, hid, oup, k, s, dil, bool(se), bool(hs)))
+        inp = oup
+    return plan, hid
+
+
+def se_inter(c):
+    return _make_divisible(c // 4)             # SELayer(channel, reduction=4), mobilenetv3.py:51-59
+
+
+def _mobilenetv3():
+    """Parameter tree of MobileNetV3Large (mobilenetv3.py:68-215) with the reference's names: features.0.{0,1} stem,
+    features.<n>.conv.<m> per InvertedResidual (activations and a missing SE are parameter-free slots), SE as
+    conv.<m>.fc.{0,2} (Linear with bias), conv.{0,1} the last 1x1 conv."""
+    enc = ParamNode()
+
+    def slot():
+        return ParamNode()
+
+    def se(c):
+        m = ParamNode()
+        m.fc = _seq([Linear(c, se_inter(c)), slot(), Linear(se_inter(c), c), slot()])
+        return m
+
+    feats = [_seq([Conv(3, 16, 3, bias=False), FrozenBN(16), slot()])]
+    plan, last = mobilenetv3_plan(16)
+    for inp, hid, oup, k, s, dil, use_se, hs in plan:
+        if inp == hid:
+            mods = [Conv(hid, hid, k, bias=False, groups=hid), FrozenBN(hid), slot(), se(hid) if use_se else slot()]
+        else:
+            mods = [Conv(inp, hid, 1, bias=False), FrozenBN(hid), slot(), Conv(hid, hid, k, bias=False, groups=hid),
+                    FrozenBN(hid), se(hid) if use_se else slot(), slot()]
+        blk = ParamNode()
+        blk.conv = _seq(mods + [Conv(hid, oup, 1, bias=False), FrozenBN(oup)])
+        feats.append(blk)
+    enc.features = _seq(feats)
+    enc.conv = _seq([Conv(plan[-1][2], last, 1, bias=False), FrozenBN(last), slot()])
+    for m in enc.modules():                                     # mobilenetv3.py:217-230
+        if isinstance(m, Conv):
+            n = m.weight.shape[2] * m.weight.shape[3] * m.weight.shape[0]
+            nn.init.normal_(m.weight, 0, math.sqrt(2.0 / n))
+        elif isinstance(m, Linear):
+            nn.init.normal_(m.weight, 0, 0.01)
+            nn.init.zeros_(m.bias)
+    return enc
+
+
+# channel counts of the four feature maps each encoder returns (what cfg.MODEL_ENCODER_DIM must list)
+ENCODER_DIMS = {"resnet50": [256, 512, 1024, 1024], "resnet101": [256, 512, 1024, 1024],
+                "resnest50": [256, 512, 1024, 1024], "resnest101": [256, 512, 1024, 1024],
+                "mobilenetv2": [24, 32, 96, 1280], "mobilenetv3": [24, 40, 112, 960], "swin_base": [128, 256, 512, 512]}
+
+
 def build_encoder_params(name):
     if name in RESNET_LAYERS:
         return _resnet(RESNET_LAYERS[name])
-    if name == "resnest101":
-        return _resnest101()
+    if name in RESNEST:
+        return _resnest(*RESNEST[name])
     if name == "mobilenetv2":
         return _mobilenetv2()
+    if name == "mobilenetv3":
+        return _mobilenetv3()
     if name == "swin_base":
         return _swin_base()
-    raise NotImplementedError(f"encoder '{name}' has no sm_90a path yet (resnet50, resnet101, resnest101, mobilenetv2, "
-                              "swin_base do)")
+    raise NotImplementedError(f"encoder '{name}' has no sm_90a path (available: {', '.join(ENCODER_DIMS)})")
 
 
 # ---------------------------------------------------------------- transformer blocks
@@ -414,6 +491,10 @@ class AOT(nn.Module):
         L = cfg.MODEL_LSTT_NUM
         if not getattr(cfg, "MODEL_FREEZE_BN", True):
             raise NotImplementedError("the H100 hot path folds FrozenBatchNorm2d; MODEL_FREEZE_BN=False is train-only")
+        dims = ENCODER_DIMS.get(encoder)
+        if dims is not None and list(cfg.MODEL_ENCODER_DIM) != dims:
+            raise ValueError(f"cfg.MODEL_ENCODER_DIM = {list(cfg.MODEL_ENCODER_DIM)} does not match encoder '{encoder}', whose "
+                             f"feature maps have {dims} channels: set cfg.MODEL_ENCODER_DIM = {dims}")
         self.encoder = build_encoder_params(encoder)
         self.encoder_projector = Conv(cfg.MODEL_ENCODER_DIM[-1], d, 1)
         self._build_lstt(cfg, d, L)

@@ -15,7 +15,7 @@ import torch
 
 from ._lib import AotbError, check, lib
 
-ACT_NONE, ACT_RELU, ACT_GELU, ACT_SILU, ACT_RELU6 = 0, 1, 2, 3, 4
+ACT_NONE, ACT_RELU, ACT_GELU, ACT_SILU, ACT_RELU6, ACT_HSWISH = 0, 1, 2, 3, 4, 5
 EW_COPY, EW_ADD, EW_MUL, EW_SILU, EW_SILU_MUL, EW_FILL = 0, 1, 2, 3, 4, 5
 
 
@@ -433,6 +433,32 @@ def splat_combine(x, att, out, radix=2, pool_stride=0, stream=None):
         raise AotbError(f"splat_combine: x {tuple(x.shape)}, att {tuple(att.shape)}, out {tuple(out.shape)}")
     check(lib().aotb_splat_combine_f32(_p(x), _nhwc_ld(x), _p(att), _p(out), _nhwc_ld(out), H, W, C, radix, int(pool_stride),
                                        _st(stream)), "aotb_splat_combine_f32")
+    return out
+
+
+def se_gate(x, w1, b1, w2, b2, gate, workspace, stream=None):
+    """Squeeze-excite gate of one image: x [1,H,W,C] NHWC (or [HW, C]), w1 [C, inter], b1 [inter], w2 [inter, C], b2 [C]
+    -> gate [C] = h_sigmoid(ReLU(mean(x) @ w1 + b1) @ w2 + b2).  `workspace` comes from splat_workspace(>= C)."""
+    _chk(x, w1, b1, w2, b2, gate)
+    x2 = x.reshape(-1, x.shape[-1]) if x.dim() == 4 else x
+    HW, ld = x2.shape[0], (_nhwc_ld(x) if x.dim() == 4 else x.stride(0))
+    C, inter = w1.shape
+    if w2.shape != (inter, C) or b1.numel() != inter or b2.numel() != C or gate.numel() != C or x.shape[-1] != C \
+            or not (w1.is_contiguous() and w2.is_contiguous() and gate.is_contiguous()):
+        raise AotbError("se_gate: shapes x [.., C], w1 [C, inter], w2 [inter, C], gate [C]")
+    check(lib().aotb_se_gate_f32(_p(x), ld, HW, C, _p(w1), _p(b1), inter, _p(w2), _p(b2), _p(gate), workspace.data_ptr(),
+                                 _st(stream)), "aotb_se_gate_f32")
+    return gate
+
+
+def gate_scale(x, gate, out, act=ACT_NONE, stream=None):
+    """out [1,H,W,C] = act(gate[c] * x [1,H,W,C]); x / out may be channel slices."""
+    _chk(x, gate, out)
+    B, H, W, C = x.shape
+    if B != 1 or tuple(out.shape) != (1, H, W, C) or gate.numel() != C:
+        raise AotbError(f"gate_scale: x {tuple(x.shape)}, gate {tuple(gate.shape)}, out {tuple(out.shape)}")
+    check(lib().aotb_gate_scale_f32(_p(x), _nhwc_ld(x), _p(gate), _p(out), _nhwc_ld(out), H * W, C, int(act), _st(stream)),
+          "aotb_gate_scale_f32")
     return out
 
 

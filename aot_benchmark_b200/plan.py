@@ -17,7 +17,8 @@ from types import SimpleNamespace as NS
 
 import torch
 
-from .model import RESNEST101_LAYERS, RESNET_LAYERS, SWIN_BASE, mobilenetv2_plan, swin_relative_position_index
+from .model import (RESNEST, RESNET_LAYERS, SWIN_BASE, mobilenetv2_plan, mobilenetv3_plan,
+                    swin_relative_position_index)
 
 
 def _signature(model):
@@ -200,20 +201,47 @@ class Plan:
             self.enc = e
         elif name == "swin_base":
             self.enc = self._swin(p)
-        elif name == "resnest101":
-            self.enc = self._resnest(p)
+        elif name == "mobilenetv3":
+            self.enc = self._mobilenetv3(p)
+        elif name in RESNEST:
+            self.enc = self._resnest(p, RESNEST[name][0])
         else:
             raise NotImplementedError(f"encoder '{name}' has no sm_90a path")
 
-    def _resnest(self, p):
-        """ResNeSt-101 (resnest/resnet.py:191-357, splat.py:15-115) weights: the deep stem as three 3x3 convs (the first over
+    def _mobilenetv3(self, p):
+        """MobileNetV3-Large (mobilenetv3.py:78-215) weights: the stem over the NHWC4 image, per block the expand conv (absent
+        in block 1), the depthwise conv and the pw-linear conv with their BN folded, and the SE as fc1 [C, inter] + bias and fc2
+        [inter, C] + bias; then the last 1x1 conv."""
+        sd = self.sd
+        e = NS(stem=self._conv_bn(p + "features.0.0", p + "features.0.1", pad_cin_to=4), blocks=[])
+        plan, _ = mobilenetv3_plan(16)
+        for idx, (inp, hid, oup, k, stride, dil, se, hs) in enumerate(plan, start=1):
+            q = f"{p}features.{idx}.conv."
+            b = NS(k=k, stride=stride, dil=dil, hs=hs, res=(stride == 1 and inp == oup), expand=None, se=None,
+                   tap=idx in (3, 6, 12))
+            if inp == hid:                       # dw, bn, act, SE slot, pw, bn: no block of the table has an SE here
+                assert not se, "MobileNetV3 block without an expand conv and with SE is not in the reference's table"
+                b.dw, b.pw = self._conv_bn(q + "0", q + "1", depthwise=True), self._conv_bn(q + "4", q + "5")
+            else:                                # pw, bn, act, dw, bn, SE slot, act, pw-linear, bn
+                b.expand = self._conv_bn(q + "0", q + "1")
+                b.dw, b.pw = self._conv_bn(q + "3", q + "4", depthwise=True), self._conv_bn(q + "7", q + "8")
+                if se:
+                    f = q + "5.fc."
+                    b.se = NS(w1=self._f(sd[f + "0.weight"].t()), b1=self._f(sd[f + "0.bias"]),
+                              w2=self._f(sd[f + "2.weight"].t()), b2=self._f(sd[f + "2.bias"]))
+            e.blocks.append(b)
+        e.last = self._conv_bn(p + "conv.0", p + "conv.1")
+        return e
+
+    def _resnest(self, p, layers):
+        """ResNeSt-50 / ResNeSt-101 (resnest/resnet.py:191-357, splat.py:15-115) weights: the deep stem as three 3x3 convs (the first over
         the NHWC4 image), per bottleneck conv1 / conv3 with bn1 / bn3 folded, the radix-2 grouped 3x3 conv of SplAtConv2d as
         one [9 * gw/2, gw] weight per group with its slice of bn0 folded (each group is one launch on channel slices), fc1 with
         bn1 folded as [gw, inter] + bias, fc2 as [inter, 2 gw] + bias, and the avg_down downsample conv with its BN folded."""
         sd = self.sd
         e = NS(stem=[self._conv_bn(p + "conv1.0", p + "conv1.1", pad_cin_to=4), self._conv_bn(p + "conv1.3", p + "conv1.4"),
                      self._conv_bn(p + "conv1.6", p + "bn1")], stages=[])
-        for li, (nblk, stride) in enumerate(zip(RESNEST101_LAYERS, (1, 2, 2)), start=1):
+        for li, (nblk, stride) in enumerate(zip(layers, (1, 2, 2)), start=1):
             blocks = []
             for bi in range(nblk):
                 q = f"{p}layer{li}.{bi}."

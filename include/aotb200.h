@@ -40,7 +40,10 @@ int aotb_set_conv_tiling(int mode);
 /* nn.Conv2d (+ folded FrozenBatchNorm2d, + residual, + activation) as im2col-free implicit GEMM.
  * networks/encoders/resnet.py:34-54,140-157; networks/layers/normalization.py:30-43;
  * networks/models/aot.py:19-21,83; networks/decoders/fpn.py:34-58.
- * in [B][H][W][ldin], w [KH*KW*Cin][Cout], out [B][Ho][Wo][ldout], res like out with ldres. */
+ * in [B][H][W][ldin], w [KH*KW*Cin][Cout], out [B][Ho][Wo][ldout], res like out with ldres.
+ * act: 0 none, 1 ReLU, 2 exact GELU, 3 SiLU, 4 ReLU6, 5 h_swish = v * relu6(v + 3) / 6 (networks/encoders/mobilenetv3.py:33-48,
+ * true division by 6).  h_swish is taken by this conv, aotb_linear_f32, aotb_dwconv_nhwc_f32 and aotb_gate_scale_f32; the
+ * tensor-core conv, the conv chain and GroupNorm accept 0-4 only. */
 int aotb_conv2d_nhwc_f32(const float* in, const float* w, const float* bias, const float* res, float* out,
                          int B, int H, int W, int Cin, int ldin, int Cout, int ldout, int ldres,
                          int KH, int KW, int stride, int pad, int dil, int act, void* stream);
@@ -135,6 +138,14 @@ int aotb_splat_attention_f32(const float* x, int ldx, int HW, int C, int radix, 
  * full-resolution sum is never written; pool_stride 0: Ho = H, Wo = W. */
 int aotb_splat_combine_f32(const float* x, int ldx, const float* att, float* out, int ldo, int H, int W, int C, int radix,
                            int pool_stride, void* stream);
+/* Squeeze-excite gate of one image (networks/encoders/mobilenetv3.py:51-65): x [HW][ldx] (C channels), gap = mean over the
+ * pixels, h = ReLU(gap @ w1 + b1) with w1 [C][inter], gate [C] = h_sigmoid(h @ w2 + b2) with w2 [inter][C].  C % 4 == 0,
+ * C <= 1024, inter <= 1024.  The same deterministic multi-CTA reduction as aotb_splat_attention_f32, on a workspace of
+ * aotb_splat_workspace_bytes(C) bytes, zero-filled before its first use and left with a zero counter by every launch. */
+int aotb_se_gate_f32(const float* x, int ldx, int HW, int C, const float* w1, const float* b1, int inter, const float* w2,
+                     const float* b2, float* gate, void* workspace, void* stream);
+/* out [HW][ldo] = act(gate[c] * x[HW][ldx]) over C channels (the SE product, then the block's activation). */
+int aotb_gate_scale_f32(const float* x, int ldx, const float* gate, float* out, int ldo, int HW, int C, int act, void* stream);
 /* nn.AvgPool2d(k, s, pad, ceil_mode, count_include_pad) in NHWC, in [B][H][W][ldin] -> out [B][Ho][Wo][ldo] with PyTorch's
  * output extent and divisor rules: networks/encoders/resnest/resnet.py:330-342 (avg_down). */
 int aotb_avgpool_nhwc_f32(const float* in, int ldin, float* out, int ldo, int B, int H, int W, int C, int k, int s, int pad,
