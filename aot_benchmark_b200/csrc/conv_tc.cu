@@ -12,11 +12,22 @@
 // Cin % 4 == 0, Cout % 64 == 0, dilation 1 (everything on the R50-AOTL path except the 11-channel conv_out;
 // the 7x7 stem runs on a 4-channel zero-padded copy of the image).
 //
-// One CTA = 128 output pixels x BN (64 | 128) output channels, 288 threads:
-//   warps 0-7  two warpgroups running the K loop of conv_tc.cuh (each gathers, splits and stores the activations of its
-//              64 pixel rows and issues the wgmma of those rows); afterwards the accumulators go through a fp32 staging
-//              tile in shared memory and the same warps run the finish (bias / residual / activation -> fp32 NHWC stores).
-//   warp 8     TMA producer for the pre-split weights (Wh, Wl as [Cout][K] fp16, K-major), STAGES-deep ring.
+// One CTA = 128 output pixels x BN (64 | 128 | 256) output channels, 384 threads in three warpgroups, warp-specialised:
+//   warps 0-7   two consumer warpgroups (64 pixel rows each).  Per K chunk they wait for the stage's "A full" and "B full"
+//               barriers, issue 4 k-steps x (Ah Wh + Al Wh + Ah Wl) as wgmma m64nBNk16 and release the stage of the
+//               previous chunk on "empty" once its MMAs have completed.  Afterwards the accumulators go through a fp32
+//               staging tile in shared memory and the same warps run the finish (bias / residual / activation -> fp32 NHWC).
+//   warps 8-11  producer warpgroup.  It gathers the fp32 activations of all 128 rows of a chunk straight from NHWC global
+//               memory (im2col is never materialised), splits them into hi = fp16(x), lo = fp16(x - hi), stores both
+//               128 x 64 half tiles 128B-swizzled and K-major, and arrives on "A full" after fence.proxy.async.  Thread 256
+//               streams the pre-split weights (Wh, Wl as [Cout][K] fp16, K-major) into the same stage by TMA.
+// The loads go through registers, not cp.async: the split needs the values in registers anyway, and an fp32 staging area
+// (32 KB per chunk in flight) does not fit beside two BN = 256 stages.  The producer keeps two half-chunks (one chunk, 32 KB
+// per CTA) of loads in flight while it splits and stores the third, which is 96 registers per thread.
+// The N tile sets how often the activations are gathered: a layer with Cout = 256 reads its input once at BN = 256 and four
+// times at BN = 64.  STAGES: 4 at BN = 64, 3 at 128, 2 at 256 (a stage is 32 KB of A plus BN * 256 bytes of B).
+#include <type_traits>
+
 #include "conv_tc.cuh"
 
 namespace aotb {
@@ -94,8 +105,9 @@ __device__ __forceinline__ void conv_finish_tile(const ConvTcArgs& a, const uint
 // already in registers (`pre`, loaded by finish_prefetch before the thread waited for the accumulator, i.e. under the tail of the
 // K loop), and inside the loop the residual rows of batch k+1 are requested before batch k is computed and stored.  The staging
 // tile is read with ld.shared so that the compiler does not have to order those reads behind the global stores.
+// Rows per batch: 4 at BN = 256, where the prefetched rows sit beside 128 accumulator registers.
 template <int BN>
-struct FinishPre { float4 b4, s4; float4 rs[8]; };
+struct FinishPre { static constexpr int B = BN == 256 ? 4 : 8; float4 b4, s4; float4 rs[B]; };
 
 template <int BN>
 __device__ __forceinline__ void finish_prefetch(const ConvTcArgs& a, int tid, int m0, int n0, FinishPre<BN>& pre) {
@@ -104,7 +116,7 @@ __device__ __forceinline__ void finish_prefetch(const ConvTcArgs& a, int tid, in
     pre.b4 = a.bias ? __ldg(reinterpret_cast<const float4*>(a.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
     pre.s4 = a.wscale ? __ldg(reinterpret_cast<const float4*>(a.wscale + n)) : make_float4(1.f, 1.f, 1.f, 1.f);
 #pragma unroll
-    for (int b = 0; b < 8; ++b) {
+    for (int b = 0; b < FinishPre<BN>::B; ++b) {
         const int m = m0 + r0 + b * RSTEP;
         pre.rs[b] = (a.res && m < a.M) ? *reinterpret_cast<const float4*>(a.res + (size_t)m * a.ldres + n)
                                        : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -114,7 +126,7 @@ __device__ __forceinline__ void finish_prefetch(const ConvTcArgs& a, int tid, in
 template <int BN>
 __device__ __forceinline__ void conv_finish_tile_pre(const ConvTcArgs& a, const uint8_t* smem, int tid, int m0, int n0,
                                                      const FinishPre<BN>& pre) {
-    constexpr int LD = BN + 4, C4 = BN / 4, RSTEP = 256 / C4, ITERS = 128 / RSTEP, B = 8;
+    constexpr int LD = BN + 4, C4 = BN / 4, RSTEP = 256 / C4, ITERS = 128 / RSTEP, B = FinishPre<BN>::B;
     static_assert(ITERS % B == 0, "finish tiling");
     const int c = (tid % C4) * 4, n = n0 + c, r0 = tid / C4;
     const uint32_t sbase = smem_u32(reinterpret_cast<const float*>(smem) + r0 * LD + c);
@@ -161,18 +173,20 @@ struct ConvSmem {
     static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
     static constexpr int STG_LD = BN + 4;              // staging tile [128][BN + 4] fp32, aliases the stages
     static_assert(128 * STG_LD * 4 <= STAGES * STAGE_BYTES, "staging tile must fit in the operand stages");
-    static constexpr int TOTAL = STAGES * STAGE_BYTES + 128 * (int)sizeof(RowInfo) + 2 * STAGES * 8 + 1024;
+    static constexpr int TOTAL = STAGES * STAGE_BYTES + 128 * (int)sizeof(RowInfo) + 3 * STAGES * 8 + 1024;
+    static_assert(TOTAL <= 227 * 1024, "shared memory of one CTA");
 };
 
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(288, 1)
+__global__ void __launch_bounds__(384, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const ConvTcArgs a) {
     using SM = ConvSmem<BN, STAGES>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     RowInfo* rinfo = reinterpret_cast<RowInfo*>(smem + STAGES * SM::STAGE_BYTES);
-    uint64_t* b_full = reinterpret_cast<uint64_t*>(rinfo + 128);
-    uint64_t* s_free = b_full + STAGES;
+    uint64_t* a_full = reinterpret_cast<uint64_t*>(rinfo + 128);    // 128 producer-thread arrivals
+    uint64_t* b_full = a_full + STAGES;                               // TMA transaction bytes
+    uint64_t* s_free = b_full + STAGES;                               // 8 consumer-warp arrivals
 
     const int tid = threadIdx.x, warp = tid >> 5;
     const int m0 = blockIdx.x * 128, n0 = blockIdx.y * BN;
@@ -182,7 +196,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
     pdl_trigger();      // the next kernel may start its prologue; it waits for this grid before reading our output
 
     if (tid == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&b_full[s], 1); mbar_init(&s_free[s], 8); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&a_full[s], 128); mbar_init(&b_full[s], 1); mbar_init(&s_free[s], 8); }
         fence_mbar_init();
     }
     if (tid < 128) {
@@ -210,60 +224,145 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
     const int nloc = max(0, min(per, a.nchunks - kbeg));     // chunks of this CTA (local index it <-> chunk kbeg + it)
 
     FinishPre<BN> pre;
-    if (warp < 8) {
-        // ======================= K loop (two warpgroups) =======================
-        const int q = tid & 15, rbase = (tid >> 7) * 64 + ((tid & 127) >> 4);   // rows rbase + i*8, i = 0..7
-        // Per-row source pointers for the current filter tap (nullptr = zero padding / out of range); recomputed only when
-        // the tap changes (never for 1x1 convs and linears, every Cin/64 chunks for 3x3), so the steady-state work per
-        // 16-byte segment is one LDG, the hi/lo split and two 8-byte swizzled STS.
-        const float* rowptr[8];
-        int cur_tap = -1;
-        auto load_chunk = [&](int kc, float4* v) {
-            int tap, c0;
-            if (cpt > 0) { tap = kc / cpt; c0 = ((kc - tap * cpt) << 6) + q * 4; }       // Cin % 64 == 0
-            else { const int k = kc * 64 + q * 4; tap = k / a.Cin; c0 = k - tap * a.Cin; }  // Cin % 4 == 0 (stem)
-            if (tap != cur_tap) {
-                cur_tap = tap;
-                const bool kvalid = tap < a.KH * a.KW;                                     // zero padding of K
-                const int ky = tap / a.KW, kx = tap - ky * a.KW;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const RowInfo ri = rinfo[rbase + i * 8];
-                    const int iy = ri.iy0 + ky, ix = ri.ix0 + kx;
-                    rowptr[i] = (kvalid && ri.valid && iy >= 0 && iy < a.H && ix >= 0 && ix < a.W)
-                                    ? a.in + (size_t)(ri.pix_base + iy * a.W + ix) * a.ldin
-                                    : nullptr;
-                }
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-                v[i] = rowptr[i] ? __ldg(reinterpret_cast<const float4*>(rowptr[i] + c0)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        };
+    // warpgroup index made warp-uniform for the compiler: wgmma in a branch it cannot prove uniform is serialised
+    const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
+    if (wg < 2) {
+        // ======================= consumers: wgmma only =======================
+        const uint64_t dA0 = smem_desc_sw128(smem_u32(smem + wg * 64 * 128));
+        const uint64_t dB0 = smem_desc_sw128(smem_u32(smem + 2 * SM::A_BYTES));
         float acc[BN / 2];
 #pragma unroll
         for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
-        conv_kloop<BN, STAGES>(acc, smem, SM::STAGE_BYTES, SM::B_BYTES, b_full, s_free, 0, nloc, kbeg, load_chunk, a.spin,
-                               tid == 0 ? prof : nullptr);
+#pragma unroll 1
+        for (int it = 0; it < nloc; ++it) {
+            const int s = it % STAGES;
+            const uint32_t ph = (it / STAGES) & 1;
+            mbar_wait_cp(&a_full[s], ph, a.spin);
+            mbar_wait_cp(&b_full[s], ph, a.spin);
+            if (it == 0 && tid == 0) stamp(3);
+            const uint64_t so = (uint64_t)((s * SM::STAGE_BYTES) >> 4);
+            const uint64_t ah = dA0 + so, al = ah + (SM::A_BYTES >> 4), bh = dB0 + so, bl = bh + (uint64_t)(SM::B_BYTES >> 4);
+            reg_fence<BN / 2>(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) {
+                wgmma_conv<BN>(acc, ah + 2 * ks, bh + 2 * ks);
+                wgmma_conv<BN>(acc, al + 2 * ks, bh + 2 * ks);
+                wgmma_conv<BN>(acc, ah + 2 * ks, bl + 2 * ks);
+            }
+            wgmma_commit();
+            reg_fence<BN / 2>(acc);
+            wgmma_wait<1>();                              // the MMAs of the previous chunk have completed: release its stage
+            if (it > 0) mbar_arrive_warp(&s_free[(it - 1) % STAGES]);
+        }
+        wgmma_wait<0>();
+        reg_fence<BN / 2>(acc);
+        if (tid == 0) stamp(4);
         if (a.splits == 1) finish_prefetch<BN>(a, tid, m0, n0, pre);      // bias + first residual rows
-        if (tid == 0) stamp(5);
-        // every MMA of both warpgroups has completed before the staging tile overwrites the operand stages
+        // every MMA of both warpgroups has completed before the staging tile overwrites the operand stages (the producer
+        // wrote nothing after the last chunk, whose stage the consumers have waited for)
         asm volatile("bar.sync 1, 256;" ::: "memory");
         conv_acc_to_staging<BN>(acc, reinterpret_cast<float*>(smem), SM::STG_LD);
-    } else if (warp == 8) {
-        // ======================= weight TMA producer =======================
-        if (elect_one()) {
-            tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
-            for (int it = 0; it < nloc; ++it) {
-                const int s = it % STAGES;
-                if (it >= STAGES) mbar_wait(&s_free[s], ((it / STAGES) - 1) & 1);
-                uint8_t* Bh = smem + s * SM::STAGE_BYTES + 2 * SM::A_BYTES;
-                mbar_arrive_expect_tx(&b_full[s], 2 * SM::B_BYTES);
-                tma_load_2d(Bh, &tmWh, &b_full[s], (kbeg + it) * 64, n0);
-                tma_load_2d(Bh + SM::B_BYTES, &tmWl, &b_full[s], (kbeg + it) * 64, n0);
+        if (tid == 0) stamp(6);
+    } else {
+        // ======================= producer: activation gather + weight TMA =======================
+        // Thread p gathers the 16-byte segment q of rows rsub + 8 i (i = 0..15) of every chunk, in two half chunks (rows
+        // [0, 64) then [64, 128)) of 8 float4.  A ring of three half-chunk buffers keeps the next two in flight.
+        const int p = tid - 256, q = p & 15, rsub = p >> 4;
+        // byte offset of this thread's 8-byte slot in the 128 x 64 half tile (128B swizzle; row & 7 == rsub)
+        const uint32_t soff = rsub * 128 + (((q >> 1) ^ rsub) << 4) + ((q & 1) << 3);
+        const float4* in4 = reinterpret_cast<const float4*>(a.in);
+        // source of row rsub + 8 i for the current filter tap, in float4 units (~0u = zero padding / out of range);
+        // recomputed only when the tap changes (never for 1x1 convs and linears, every Cin/64 chunks for 3x3)
+        uint32_t off[16];
+        int cur_tap = -1, c4 = 0;
+        if (p == 0) { tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl); }
+        auto load_half = [&](int h, auto part_c, float4* v) {
+            constexpr int part = decltype(part_c)::value;
+            if (part == 0) {
+                const int kc = kbeg + (h >> 1);
+                int tap, c0;
+                if (cpt > 0) { tap = kc / cpt; c0 = ((kc - tap * cpt) << 6) + q * 4; }       // Cin % 64 == 0
+                else { const int k = kc * 64 + q * 4; tap = k / a.Cin; c0 = k - tap * a.Cin; }  // Cin % 4 == 0 (stem)
+                c4 = c0 >> 2;
+                if (tap != cur_tap) {
+                    cur_tap = tap;
+                    const bool kvalid = tap < a.KH * a.KW;                                     // zero padding of K
+                    const int ky = tap / a.KW, kx = tap - ky * a.KW;
+#pragma unroll
+                    for (int i = 0; i < 16; ++i) {
+                        const RowInfo ri = rinfo[rsub + i * 8];
+                        const int iy = ri.iy0 + ky, ix = ri.ix0 + kx;
+                        off[i] = (kvalid && ri.valid && iy >= 0 && iy < a.H && ix >= 0 && ix < a.W)
+                                     ? (uint32_t)(((size_t)(ri.pix_base + iy * a.W + ix) * a.ldin) >> 2)
+                                     : ~0u;
+                    }
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const uint32_t o = off[part * 8 + i];
+                v[i] = o != ~0u ? __ldg(in4 + ((size_t)o + c4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+        };
+        auto store_half = [&](int h, auto part_c, const float4* v) {
+            constexpr int part = decltype(part_c)::value;
+            const int it = h >> 1, s = it % STAGES;
+            uint8_t* stage = smem + s * SM::STAGE_BYTES;
+            if (part == 0) {
+                if (it >= STAGES) mbar_wait_cp(&s_free[s], ((it / STAGES) - 1) & 1, a.spin);
+                if (p == 0) {
+                    uint8_t* Bh = stage + 2 * SM::A_BYTES;
+                    mbar_arrive_expect_tx(&b_full[s], 2 * SM::B_BYTES);
+                    tma_load_2d(Bh, &tmWh, &b_full[s], (kbeg + it) * 64, n0);
+                    tma_load_2d(Bh + SM::B_BYTES, &tmWl, &b_full[s], (kbeg + it) * 64, n0);
+                }
+            }
+            uint8_t* Ah = stage + part * 64 * 128 + soff;
+            uint8_t* Al = Ah + SM::A_BYTES;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const __half2 h0 = __floats2half2_rn(v[i].x, v[i].y), h1 = __floats2half2_rn(v[i].z, v[i].w);
+                const __half2 l0 = __floats2half2_rn(v[i].x - __low2float(h0), v[i].y - __high2float(h0));
+                const __half2 l1 = __floats2half2_rn(v[i].z - __low2float(h1), v[i].w - __high2float(h1));
+                uint2 ph, pl;
+                ph.x = *reinterpret_cast<const uint32_t*>(&h0); ph.y = *reinterpret_cast<const uint32_t*>(&h1);
+                pl.x = *reinterpret_cast<const uint32_t*>(&l0); pl.y = *reinterpret_cast<const uint32_t*>(&l1);
+                *reinterpret_cast<uint2*>(Ah + i * 1024) = ph;      // row part*64 + i*8 + rsub
+                *reinterpret_cast<uint2*>(Al + i * 1024) = pl;
+            }
+            if (part == 1) {
+                fence_proxy_async();      // generic-proxy smem writes -> visible to the tensor core (async proxy)
+                mbar_arrive(&a_full[s]);
+                if (it == 0 && p == 0) stamp(2);
+            }
+        };
+        using P0 = std::integral_constant<int, 0>;
+        using P1 = std::integral_constant<int, 1>;
+        const int nh = 2 * nloc;      // half chunks; h -> buffer h % 3, part h % 2
+        float4 v0[8], v1[8], v2[8];
+        if (nh > 0) { load_half(0, P0{}, v0); load_half(1, P1{}, v1); }
+#pragma unroll 1
+        for (int h = 0; h < nh; h += 6) {
+            if (h + 2 < nh) load_half(h + 2, P0{}, v2);
+            store_half(h, P0{}, v0);
+            if (h + 3 < nh) load_half(h + 3, P1{}, v0);
+            store_half(h + 1, P1{}, v1);
+            if (h + 2 < nh) {
+                if (h + 4 < nh) load_half(h + 4, P0{}, v1);
+                store_half(h + 2, P0{}, v2);
+                if (h + 5 < nh) load_half(h + 5, P1{}, v2);
+                store_half(h + 3, P1{}, v0);
+            }
+            if (h + 4 < nh) {
+                if (h + 6 < nh) load_half(h + 6, P0{}, v0);
+                store_half(h + 4, P0{}, v1);
+                if (h + 7 < nh) load_half(h + 7, P1{}, v1);
+                store_half(h + 5, P1{}, v2);
             }
         }
+        if (p == 0) stamp(5);
     }
-    if (tid == 0) stamp(6);
     // Finish: CTA z of a split-K cluster owns rows [z*128/S, (z+1)*128/S) of the tile and reads that slice of every
     // peer's staging buffer through distributed shared memory, summing in rank order (deterministic); without split-K
     // (S = 1) it is the CTA's own buffer.  Then bias / residual / activation and coalesced row stores.  No global
@@ -316,7 +415,7 @@ static int launch_conv_tc(const CUtensorMap& th, const CUtensorMap& tl, const Co
         configured = true;
     }
     dim3 grid(cdiv(a.M, 128), a.Cout / BN, a.splits);
-    launch_cluster(conv_tc_kernel<BN, STAGES>, dim3(grid), dim3(288), smem, st, a.splits, th, tl, a);
+    launch_cluster(conv_tc_kernel<BN, STAGES>, dim3(grid), dim3(384), smem, st, a.splits, th, tl, a);
     return check_launch("aotb_conv2d_nhwc_tc");
 }
 
@@ -344,6 +443,8 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
                      ((uintptr_t)out % 16 == 0) && (!res || (uintptr_t)res % 16 == 0) && (!bias || (uintptr_t)bias % 16 == 0) &&
                      (!wscale || (uintptr_t)wscale % 16 == 0),
                  "aotb_conv2d_nhwc_tc: 16-byte alignment required");
+    // the producer addresses the input in 32-bit float4 offsets (~0u marks padding)
+    AOTB_REQUIRE((size_t)B * H * W * ldin / 4 < 0xFFFFFFFFull, "aotb_conv2d_nhwc_tc: input larger than 2^32 float4");
     tc::ConvTcArgs a;
     a.in = in; a.bias = bias; a.wscale = wscale; a.res = res; a.out = out;
     a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.ldin = ldin;
@@ -355,20 +456,23 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     const int K = ((KH * KW * Cin + 63) / 64) * 64;   // weights are zero-padded to a multiple of 64 along K
     a.nchunks = K / 64;
     a.act = act;
-    // Tile policy: pick the N tile (64 / 128 dividing Cout) and the split-K cluster size (1 / 2 / 4 / 8) that minimise
-    //     T = waves * (ramp + chunks_per_cta * t_chunk[BN] + t_finish[BN])
-    // over the 132 SMs of an H100 (one CTA per SM).  The per-chunk and finish costs are in units of one BN = 64 chunk and
-    // proportional to the tile's MMA work and bytes.  Split-K is only used to fill a partial wave.  Checked against
-    // scripts/conv_sweep.py on an H100 (80GB HBM3, 700 W): over the 20 conv / linear shapes of an R50-AOTL 480p frame the
-    // policy's tiles take 1130 us in total against 1117 us for the best measured tiling of each shape.  Bit 0 of the tuning
-    // mask ("narrow") selects the simpler heuristic instead.
+    // Tile policy: pick the N tile (64 / 128 / 256 dividing Cout) and the split-K cluster size (1 / 2 / 4 / 8) that minimise
+    //     T = waves * (ramp + chunks_per_cta * t_chunk[BN] + t_finish[BN]),   t_chunk[BN] = max(kGather, BN / 64)
+    // over the 132 SMs of an H100 (one CTA per SM).  Costs are in units of the MMAs of one BN = 64 chunk.  The producer's
+    // gather of a chunk (32 KB of fp32 activations) overlaps the MMAs and takes kGather units whatever BN is, so narrow
+    // tiles are gather-bound and BN = 256 is MMA-bound.  Split-K is only used to fill a partial wave.  kGather was fitted
+    // with scripts/conv_sweep.py on an H100 (80GB HBM3, 700 W): over the 20 conv / linear shapes of an R50-AOTL 480p frame
+    // the policy's tiles take 632 us in total against 632 us for the best measured tiling of each shape.  Bit 0 of the
+    // tuning mask ("narrow") selects the simpler heuristic instead.
     const int mt = cdiv(a.M, 128);
     int BN = 64, best_s = 1;
+    const float kGather = 2.5f;
     if ((tc::g_conv_tiling & 1) == 0) {
         float best = 1e30f;
-        const int bns[2] = {128, 64};
-        const float t_chunk[2] = {2.0f, 1.0f}, t_fin[2] = {4.0f, 2.0f};
-        for (int bi = 0; bi < 2; ++bi) {
+        const int bns[3] = {256, 128, 64};
+        const float t_chunk[3] = {fmaxf(kGather, 4.0f), fmaxf(kGather, 2.0f), fmaxf(kGather, 1.0f)};
+        const float t_fin[3] = {8.0f, 4.0f, 2.0f};
+        for (int bi = 0; bi < 3; ++bi) {
             if (Cout % bns[bi]) continue;
             for (int sp = 1; sp <= 8; sp <<= 1) {
                 if (sp > a.nchunks) break;
@@ -391,7 +495,7 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     const int force_bn = (tc::g_conv_tiling >> 4) & 15, force_s = (tc::g_conv_tiling >> 8) & 15;
     if (force_bn) {
         BN = 32 << force_bn;
-        AOTB_REQUIRE((BN == 64 || BN == 128) && Cout % BN == 0, "aotb_conv2d_nhwc_tc: forced tile %d invalid", BN);
+        AOTB_REQUIRE((BN == 64 || BN == 128 || BN == 256) && Cout % BN == 0, "aotb_conv2d_nhwc_tc: forced tile %d invalid", BN);
     }
     a.splits = force_bn ? 1 : best_s;
     const int ctas = mt * (Cout / BN);
@@ -412,6 +516,7 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     if ((rc = tc::make_tmap_weights(&th, wh, K, Cout, BN)) != AOTB_OK) return rc;
     if ((rc = tc::make_tmap_weights(&tl, wl, K, Cout, BN)) != AOTB_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
+    if (BN == 256) return tc::launch_conv_tc<256, 2>(th, tl, a, st);
     if (BN == 128) return tc::launch_conv_tc<128, 3>(th, tl, a, st);
-    return tc::launch_conv_tc<64, 3>(th, tl, a, st);
+    return tc::launch_conv_tc<64, 4>(th, tl, a, st);
 }

@@ -1,5 +1,5 @@
-// K loop of the tensor-core implicit-GEMM convolution, shared by the per-layer kernel (conv_tc.cu) and the persistent chain
-// kernel (conv_chain.cu).  A 128-pixel x BN-channel output tile is computed by two consumer warpgroups, 64 pixel rows each.
+// K loop of the persistent conv chain kernel (conv_chain.cu), plus the pieces the warp-specialised per-layer kernel
+// (conv_tc.cu) shares with it.  A 128-pixel x BN-channel output tile is computed by two warpgroups, 64 pixel rows each.
 // Per 64-deep K chunk a warpgroup
 //   - gathers the fp32 activations of ITS 64 rows straight from NHWC global memory (the caller's load_chunk: im2col is never
 //     materialised), splits every value into hi = fp16(x), lo = fp16(x - hi) and stores both 64 x 64 half tiles into the
@@ -20,7 +20,8 @@ constexpr int CONV_A_BYTES = 128 * 128;        // one 128 x 64 half tile (both w
 
 template <int BN>
 __device__ __forceinline__ void wgmma_conv(float* acc, uint64_t a, uint64_t b) {
-    if (BN == 128) wgmma_ss_n128(acc, a, b, 1u);
+    if (BN == 256) wgmma_ss_n256(acc, a, b, 1u);
+    else if (BN == 128) wgmma_ss_n128(acc, a, b, 1u);
     else wgmma_ss_n64(acc, a, b, 1u);
 }
 

@@ -33,7 +33,8 @@ SHAPES = [  # name, H, W, Cin, Cout, K, stride, pad
     ("lstt linear 1024->256", 1674, 1, 1024, 256, 1, 1, 0),
 ]
 REP = 20
-NAMES = ["prologue", "A0 stored", "stage0 ready", "last MMA issued", "acc complete", "staged", "exit", "finish start",
+# stamp slots 1..9: consumer thread 0 except "A0 stored" and "producer done" (producer thread 256)
+NAMES = ["prologue", "A0 stored", "stage0 ready", "acc complete", "producer done", "staged", "exit", "finish start",
          "finish stored"]
 
 

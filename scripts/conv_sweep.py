@@ -57,7 +57,7 @@ def main():
         fn = lambda: ops.conv2d_tc(x, wh, wl, b, out, KH=K, KW=K, stride=s, pad=p, act=1)  # noqa: E731
         lib().aotb_set_conv_tiling(0)
         row["us"]["policy"] = round(time_graph(fn), 2)
-        for bi, BN in ((1, 64), (2, 128)):
+        for bi, BN in ((1, 64), (2, 128), (3, 256)):
             if Cout % BN:
                 continue
             for S in (1, 2, 4, 8):
