@@ -5,7 +5,8 @@ hand-written sm_90a kernels from libaotb200.so on ``stream`` (a raw cudaStream_t
 torch's current stream) and raises ``AotbError`` on failure -- there is no eager fallback.
 
 Layout conventions: activations are NHWC ``[B,H,W,C]`` or token matrices ``[rows, C]`` whose last
-stride is 1; channel-sliced views are fine (the row stride is passed as ``ld``).
+stride is 1; channel-sliced views are fine (the row stride is passed as ``ld``), except where a wrapper says its
+operands must be contiguous (the label-map, logit post-processing and ID-embedding kernels), and there it checks.
 """
 from __future__ import annotations
 
@@ -540,10 +541,28 @@ def local_attention_tile(q, k, v, relk_w, relk_b, relv_t, out, h, w, H, stream=N
     return out
 
 
-def id_embed(mask, wt, bias, out, C, nid, ksize, stride, pad, ln_gamma=None, ln_beta=None, stream=None):
-    """mask [Hm, Wm] float ids -> out [ho*wo, C]."""
-    _chk(mask, wt, bias, out, ln_gamma, ln_beta)
+def _id_embed_check(name, mask, table, table_shape, bias, out, C, ksize, stride, pad, ln_gamma, ln_beta):
+    """The mask is read as a dense [Hm, Wm] map and the weight table as a dense array of `table_shape`; out [ho*wo, C] may
+    have a row stride above C.  -> (Hm, Wm)."""
+    _chk(mask, table, bias, out, ln_gamma, ln_beta)
+    if mask.dim() != 2 or not mask.is_contiguous():
+        raise AotbError(f"{name}: mask must be a contiguous [Hm, Wm] map, got shape {tuple(mask.shape)}, "
+                        f"strides {mask.stride()}")
     Hm, Wm = mask.shape
+    ho, wo = (Hm + 2 * pad - ksize) // stride + 1, (Wm + 2 * pad - ksize) // stride + 1
+    if tuple(table.shape) != tuple(table_shape) or not table.is_contiguous():
+        raise AotbError(f"{name}: weight table must be a contiguous {list(table_shape)}, got {tuple(table.shape)}")
+    if bias.numel() != C or any(t is not None and t.numel() != C for t in (ln_gamma, ln_beta)):
+        raise AotbError(f"{name}: bias and LayerNorm parameters need {C} entries")
+    if out.dim() != 2 or tuple(out.shape) != (ho * wo, C):
+        raise AotbError(f"{name}: out must be [{ho * wo}, {C}] for a {Hm}x{Wm} mask, got {tuple(out.shape)}")
+    return Hm, Wm
+
+
+def id_embed(mask, wt, bias, out, C, nid, ksize, stride, pad, ln_gamma=None, ln_beta=None, stream=None):
+    """mask [Hm, Wm] float ids (contiguous) -> out [ho*wo, C]; wt [ksize*ksize*nid, C]."""
+    Hm, Wm = _id_embed_check("id_embed", mask, wt, (ksize * ksize * nid, C), bias, out, C, ksize, stride, pad, ln_gamma,
+                             ln_beta)
     check(lib().aotb_id_embed_f32(_p(mask), Hm, Wm, _p(wt), _p(bias), _p(ln_gamma), _p(ln_beta), _p(out),
                                   out.stride(0), C, nid, ksize, stride, pad, _st(stream)), "aotb_id_embed_f32")
     return out
@@ -551,16 +570,30 @@ def id_embed(mask, wt, bias, out, C, nid, ksize, stride, pad, ln_gamma=None, ln_
 
 def id_embed_runs(mask, wp, bias, out, C, nid, ksize, stride, pad, ln_gamma=None, ln_beta=None, stream=None):
     """Run-length form of id_embed; wp [ksize, ksize+1, nid, C] exclusive prefix sums along kx."""
-    _chk(mask, wp, bias, out, ln_gamma, ln_beta)
-    Hm, Wm = mask.shape
+    Hm, Wm = _id_embed_check("id_embed_runs", mask, wp, (ksize, ksize + 1, nid, C), bias, out, C, ksize, stride, pad,
+                             ln_gamma, ln_beta)
     check(lib().aotb_id_embed_runs_f32(_p(mask), Hm, Wm, _p(wp), _p(bias), _p(ln_gamma), _p(ln_beta), _p(out),
                                        out.stride(0), C, nid, ksize, stride, pad, _st(stream)), "aotb_id_embed_runs_f32")
     return out
 
 
+def _dense_maps(name, t, shape3):
+    """t must be one contiguous [..., a, b, c] map (leading dims of size 1) with the given trailing shape (None: any)."""
+    if t.dim() < 3 or t.numel() != t.shape[-3] * t.shape[-2] * t.shape[-1] or not t.is_contiguous() \
+            or any(want is not None and got != want for got, want in zip(t.shape[-3:], shape3)):
+        want = "x".join("*" if v is None else str(v) for v in shape3)
+        raise AotbError(f"{name}: need one contiguous [{want}] map, got shape {tuple(t.shape)}, strides {t.stride()}")
+
+
 def logits_postproc(logits_nhwc, lowres_nchw, out_nchw, obj_num, align_corners, stream=None):
+    """logits_nhwc [h, w, NC] -> lowres_nchw [NC, h, w] (ids > obj_num set to -1e10) and, if given, out_nchw [NC, Ho, Wo]
+    bilinearly upsampled; all three contiguous (leading dims of size 1)."""
     _chk(logits_nhwc, lowres_nchw, out_nchw)
+    _dense_maps("logits_postproc logits", logits_nhwc, (None, None, None))
     h, w, NC = logits_nhwc.shape[-3:]
+    _dense_maps("logits_postproc lowres", lowres_nchw, (NC, h, w))
+    if out_nchw is not None:
+        _dense_maps("logits_postproc out", out_nchw, (NC, None, None))
     Ho, Wo = (out_nchw.shape[-2], out_nchw.shape[-1]) if out_nchw is not None else (0, 0)
     check(lib().aotb_logits_postproc_f32(_p(logits_nhwc), _p(lowres_nchw), _p(out_nchw), h, w, NC, obj_num, Ho, Wo,
                                          1 if align_corners else 0, _st(stream)), "aotb_logits_postproc_f32")
@@ -568,9 +601,13 @@ def logits_postproc(logits_nhwc, lowres_nchw, out_nchw, obj_num, align_corners, 
 
 
 def logits_argmax(lowres_nchw, label, align_corners, stream=None):
+    """lowres_nchw [NC, h, w] -> label [Ho, Wo] = argmax over NC of the bilinear upsample; both contiguous."""
     _chk(lowres_nchw, label)
+    _dense_maps("logits_argmax lowres", lowres_nchw, (None, None, None))
     NC, h, w = lowres_nchw.shape[-3:]
     Ho, Wo = label.shape[-2:]
+    if label.numel() != Ho * Wo or not label.is_contiguous():
+        raise AotbError(f"logits_argmax: label must be one contiguous [Ho, Wo] map, got {tuple(label.shape)}")
     check(lib().aotb_logits_argmax_f32(_p(lowres_nchw), _p(label), h, w, NC, Ho, Wo, 1 if align_corners else 0,
                                        _st(stream)), "aotb_logits_argmax_f32")
     return label
@@ -635,16 +672,26 @@ def label_to_u8(label, out_u8, stream=None):
 
 
 def nearest_resize(x, out, stream=None):
+    """x [H, W] -> out [Ho, Wo] (F.interpolate(mode='nearest')); both one contiguous map (leading dims of size 1)."""
     _chk(x, out)
     H, W = x.shape[-2:]
     Ho, Wo = out.shape[-2:]
+    for t, n in ((x, H * W), (out, Ho * Wo)):
+        if t.numel() != n or not t.is_contiguous():
+            raise AotbError(f"nearest_resize: need contiguous single maps, got {tuple(t.shape)} with strides {t.stride()}")
     check(lib().aotb_nearest_resize_f32(_p(x), _p(out), H, W, Ho, Wo, _st(stream)), "aotb_nearest_resize_f32")
     return out
 
 
 def bank_append(src, bank, offset, offset_dev=None, stream=None):
+    """bank[offset + r, :cols] = src[r] for the rows of src [rows, cols]; the offset is `offset` or, if given, the int32
+    device counter `offset_dev` (read when the kernel runs, so only the host offset can be checked here)."""
     _chk(src, bank)
     rows, cols = src.shape
+    if bank.dim() != 2 or cols > bank.shape[1] or rows > bank.shape[0] or \
+            (offset_dev is None and not 0 <= int(offset) <= bank.shape[0] - rows):
+        raise AotbError(f"bank_append: {rows} x {cols} rows at offset {int(offset) if offset_dev is None else 'on device'} "
+                        f"do not fit a bank of {tuple(bank.shape)}")
     check(lib().aotb_bank_append_f32(_p(src), src.stride(0), _p(bank), bank.stride(0), rows, cols, int(offset),
                                      offset_dev.data_ptr() if offset_dev is not None else None, _st(stream)),
           "aotb_bank_append_f32")
