@@ -368,11 +368,17 @@ def layernorm(x, gamma, beta, out, add=None, out2=None, stream=None):
 
 
 def window_attention(qkv, qkv_bias, rel_bias, out, H, W, heads, shift, window=7, stream=None):
-    """Swin (S)W-MSA core: qkv [H*W, 3C], rel_bias [heads, 49, 49], out [H*W, C]."""
+    """Swin (S)W-MSA core: qkv [H*W, 3C], qkv_bias [3C], rel_bias [heads, 49, 49], out [H*W, C]."""
     _chk(qkv, qkv_bias, rel_bias, out)
     C = out.shape[1]
-    if qkv.shape[0] != H * W or qkv.shape[1] != 3 * C or out.shape[0] != H * W or not rel_bias.is_contiguous():
-        raise AotbError("window_attention: qkv must be [H*W, 3C], out [H*W, C], rel_bias contiguous")
+    if qkv.shape[0] != H * W or qkv.shape[1] != 3 * C or out.shape[0] != H * W:
+        raise AotbError("window_attention: qkv must be [H*W, 3C], out [H*W, C]")
+    # the kernel reads rel_bias[head][i][j] and qkv_bias[2C + head * head_dim + c] densely
+    T = window * window
+    if tuple(rel_bias.shape) != (heads, T, T) or not rel_bias.is_contiguous():
+        raise AotbError(f"window_attention: rel_bias must be contiguous [{heads}, {T}, {T}], got {tuple(rel_bias.shape)}")
+    if qkv_bias.numel() != 3 * C or not qkv_bias.is_contiguous():
+        raise AotbError(f"window_attention: qkv_bias must be contiguous with {3 * C} elements, got {qkv_bias.numel()}")
     check(lib().aotb_window_attention_f32(_p(qkv), qkv.stride(0), _p(qkv_bias), _p(rel_bias), _p(out), out.stride(0),
                                           H, W, C, heads, window, shift, _st(stream)), "aotb_window_attention_f32")
     return out
@@ -645,8 +651,8 @@ def preprocess_bgr_u8(img_u8, out, taps=None, flip=False, stream=None):
     if img_u8.dtype != torch.uint8 or not img_u8.is_cuda or not img_u8.is_contiguous() or img_u8.dim() != 3 or img_u8.shape[2] != 3:
         raise AotbError("preprocess_bgr_u8: image must be a contiguous uint8 CUDA tensor [H, W, 3]")
     _chk(out)
-    if not out.is_contiguous():
-        raise AotbError("preprocess_bgr_u8: out must be contiguous [1, 3, Ho, Wo]")
+    if out.dim() != 4 or tuple(out.shape[:2]) != (1, 3) or not out.is_contiguous():   # the kernel writes 3 * Ho * Wo floats
+        raise AotbError(f"preprocess_bgr_u8: out must be contiguous [1, 3, Ho, Wo], got {tuple(out.shape)}")
     H, W = int(img_u8.shape[0]), int(img_u8.shape[1])
     Ho, Wo = int(out.shape[-2]), int(out.shape[-1])
     if taps is None:
@@ -656,6 +662,8 @@ def preprocess_bgr_u8(img_u8, out, taps=None, flip=False, stream=None):
         if ix.dtype != torch.int32 or iy.dtype != torch.int32 or cx.dtype != torch.float32 or cy.dtype != torch.float32 \
                 or tuple(ix.shape) != (Wo, 4) or tuple(cx.shape) != (Wo, 4) or tuple(iy.shape) != (Ho, 4) or tuple(cy.shape) != (Ho, 4):
             raise AotbError("preprocess_bgr_u8: taps must be (int32 [Wo,4], fp32 [Wo,4], int32 [Ho,4], fp32 [Ho,4])")
+        if not all(t.is_cuda and t.is_contiguous() for t in taps):
+            raise AotbError("preprocess_bgr_u8: tap tables must be contiguous CUDA tensors")
         ptrs = tuple(t.data_ptr() for t in (ix, cx, iy, cy))
     check(lib().aotb_preprocess_bgr_u8(img_u8.data_ptr(), H, W, ptrs[0], ptrs[1], ptrs[2], ptrs[3], _p(out), Ho, Wo,
                                        1 if flip else 0, _st(stream)), "aotb_preprocess_bgr_u8")
