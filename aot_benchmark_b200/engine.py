@@ -1166,7 +1166,10 @@ class AOTEngine(nn.Module):
             ops.logits_postproc(lg, bufs[0], bufs[1], obj, P.align_corners, stream=st)
             return bufs
 
-        lo, out = self.graphs.run(("dec", size, obj, self.curr_enc_embs.nhwc[0].data_ptr()), body)
+        # keyed on every encoder map the body reads: after restart_engine() a pooled sub-engine can decode the maps of a
+        # different encoder, and the allocator may hand back only some of the blocks the captured graph points at
+        enc_ptrs = tuple(t.data_ptr() for t in self.curr_enc_embs.nhwc[:3])
+        lo, out = self.graphs.run(("dec", size, obj) + enc_ptrs, body)
         self.pred_id_logits = lo
         return lo if out is None else out
 

@@ -49,6 +49,8 @@ class OracleConfig:
         "aotl": ("aot", "mobilenetv2", [24, 32, 96, 1280], 3, True, 5),         # configs/models/aotl.py:9-12
         "r50_aotl": ("aot", "resnet50", [256, 512, 1024, 1024], 3, True, 5),    # configs/models/r50_aotl.py:7-16
         "deaott": ("deaot", "mobilenetv2", [24, 32, 96, 1280], 1, True, 9999),  # configs/models/deaott.py
+        "deaots": ("deaot", "mobilenetv2", [24, 32, 96, 1280], 2, True, 9999),  # configs/models/deaots.py
+        "deaotb": ("deaot", "mobilenetv2", [24, 32, 96, 1280], 3, True, 9999),  # configs/models/deaotb.py
         "deaotl": ("deaot", "mobilenetv2", [24, 32, 96, 1280], 3, True, 5),     # configs/models/deaotl.py
         "r50_deaotl": ("deaot", "resnet50", [256, 512, 1024, 1024], 3, True, 5),  # configs/models/r50_deaotl.py
         "swinb_aotl": ("aot", "swin_base", [128, 256, 512, 512], 3, False, 5),   # configs/models/swinb_aotl.py:9-18
@@ -786,8 +788,8 @@ class OracleInferEngine:
     (:515-545) and the per-engine logits are merged by soft_logit_aggregation (:565-582)."""
 
     def __init__(self, weights: Dict[str, Tensor], cfg, long_term_mem_gap: Optional[int] = None,
-                 short_term_mem_skip: int = 1, dtype=torch.float32):
-        self.weights, self.cfg, self.dtype = weights, cfg, dtype
+                 short_term_mem_skip: int = 1, dtype=torch.float32, device="cpu"):
+        self.weights, self.cfg, self.dtype, self.device = weights, cfg, dtype, device
         self.long_term_mem_gap = cfg.TEST_LONG_TERM_MEM_GAP if long_term_mem_gap is None else long_term_mem_gap
         self.short_term_mem_skip = short_term_mem_skip
         self.max_aot_obj_num = cfg.MODEL_MAX_OBJ_NUM
@@ -827,7 +829,7 @@ class OracleInferEngine:
         need = max(math.ceil(obj_nums / self.max_aot_obj_num), 1)
         while need > len(self.aot_engines):
             self.aot_engines.append(OracleEngine(self.weights, self.cfg, self.long_term_mem_gap,
-                                                 self.short_term_mem_skip, self.dtype))
+                                                 self.short_term_mem_skip, self.dtype, device=self.device))
         masks, nums = self.separate_mask(mask, obj_nums)
         for eng, m, n in zip(self.aot_engines, masks, nums):
             # the reference encodes the image once and hands the embeddings on (:600-607); the oracle engines

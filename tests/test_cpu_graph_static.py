@@ -126,6 +126,57 @@ def test_captured_bodies_are_static_across_frames_bank_growth_and_videos(monkeyp
         O.run_video(eng, frames, mask, 2, (H - 16, W - 16))
 
 
+def _sub_engine_logits(eng, frames, mask, objs, out_size):
+    """run_video, keeping the merged logits and every sub-engine's pred_id_logits of every frame."""
+    subs = []
+    on_frame = lambda t, logit, label: subs.append([logit.clone()] + [e.pred_id_logits.clone() for e in eng.aot_engines])
+    with torch.no_grad():
+        O.run_video(eng, frames, mask, objs, out_size, on_frame=on_frame)
+    return subs
+
+
+@pytest.mark.parametrize("model_name", ["aott", "deaott"])
+def test_sub_engine_reuse_across_videos_with_a_recycled_encoder_block(monkeypatch, model_name):
+    """restart_engine() pools the sub-engines and the next video pops them in order, so in (A, 20 objects) -> (B, 3) ->
+    (A, 20) the first video's follower owns the encoder in the third one, with a fresh _Encoder but its old workspace
+    and graphs (same geometry, and 10 objects in both roles, so its decode graph's key can match).  Stand-in for the
+    allocator handing back SOME of the freed blocks: the new encoder gets the old 4x feature tensor back and fresh 8x /
+    16x ones.  Every graph the new owner replays must then read the new encoder's maps, and every video must equal a
+    fresh engine running it alone."""
+    from aot_benchmark_b200 import engine
+    _install(monkeypatch)
+    sd = OW.build_state_dict(model_name, seed=4)
+    A, B = (97, 129), (129, 177)
+    seq = [(A, 20), (B, 3), (A, 20), (A, 3), (B, 14)]
+    clips = [O.synthetic_video(5, h, w, objs, seed=50 + i) for i, ((h, w), objs) in enumerate(seq)]
+    eng = _engine(model_name, sd, 2)
+    got = [_sub_engine_logits(eng, *clips[0], 20, A)]
+    owner, follower = eng.aot_engines
+    old_enc, old_x4 = owner._enc, owner.curr_enc_embs.nhwc[0]
+    x4_key = next(k for k, v in old_enc.bufs.items() if v is old_x4)
+    alloc = engine._Encoder._buf
+
+    def recycled_buf(self, key, shape):
+        if self is not old_enc and key == x4_key and key not in self.bufs and tuple(shape) == tuple(old_x4.shape):
+            self.bufs[key] = old_x4                 # the freed 4x block comes back; 8x / 16x are new addresses
+        return alloc(self, key, shape)
+    monkeypatch.setattr(engine._Encoder, "_buf", recycled_buf)
+    for i in range(1, len(seq)):
+        (h, w), objs = seq[i]
+        got.append(_sub_engine_logits(eng, *clips[i], objs, (h, w)))
+        if i == 2:
+            assert eng.aot_engines[0] is follower and follower._enc is not old_enc
+            assert follower.curr_enc_embs.nhwc[0] is old_x4 and follower._ws_key is not None
+    assert TracingGraphCache.replays > 20
+    for i, ((h, w), objs) in enumerate(seq):
+        alone = _sub_engine_logits(_engine(model_name, sd, 2), *clips[i], objs, (h, w))
+        assert len(alone) == len(got[i])
+        for f, (a, b) in enumerate(zip(got[i], alone)):
+            assert len(a) == len(b) == 1 + (objs + 9) // 10
+            for j, (x, y) in enumerate(zip(a, b)):
+                assert torch.equal(x, y), f"video {i + 1}, frame {f + 1}, {'merged' if j == 0 else f'sub-engine {j - 1}'}"
+
+
 def test_tracer_catches_a_per_video_tensor(monkeypatch):
     """The tracer itself: re-creating the position table per video (the round-2 bug) must be reported."""
     from aot_benchmark_b200 import engine
