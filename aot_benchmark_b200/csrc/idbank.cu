@@ -12,6 +12,8 @@
 //     reference's prepend -- softmax attention is permutation invariant over keys).
 #include "common.cuh"
 
+#include <cuda_fp16.h>
+
 namespace aotb {
 
 // weights re-laid out as wt[(ky*KW + kx) * NID + id][C]
@@ -295,6 +297,59 @@ __global__ void bank_append_kernel(const float* __restrict__ src, int lds, float
 __global__ void counter_add_kernel(int* ctr, int delta) {
     pdl_sync(); *ctr += delta; }
 
+// Bounded bank (a pinned first frame + a FIFO ring of the newest frames): one launch stores a memory frame's K and V rows into
+// every copy of the bank the attention kernels read, at the ring's device-resident write offset.
+struct RingStoreArgs {
+    const float* src[2];    // K, V rows [rows][ld]
+    float* bank[2];         // fp32 banks [cap_rows][ldb] (nullptr: no such copy)
+    __half* packed[2];      // split-fp16 banks [cols / 32][cap_rows][64] (nullptr: no such copy)
+    int ld[2], ldb[2], c4[2];   // c4: float4 groups per row
+};
+
+// One thread per (row, 4 channels) of K then V: the source is read once; the packed rows are the bytes of pack_rows64_kernel
+// with div == 1 (hi = fp16(x), lo = fp16(x - hi), [hi(32) | lo(32)] per 32-channel chunk).
+__global__ void __launch_bounds__(256) bank_ring_store_kernel(const RingStoreArgs a, int rows, int cap_rows,
+                                                              const int* __restrict__ write) {
+    pdl_sync();
+    const int off = *write;
+    if (off < 0 || off + rows > cap_rows) return;      // never write outside the bank, whatever the counter holds
+    const int per_row = a.c4[0] + a.c4[1];
+    const size_t total = (size_t)rows * per_row;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int r = i / per_row;
+        int j = i - (size_t)r * per_row;
+        const bool isv = j >= a.c4[0];                    // selects, not indexing: the arguments stay in constant memory
+        if (isv) j -= a.c4[0];
+        const float* src = isv ? a.src[1] : a.src[0];
+        float* bank = isv ? a.bank[1] : a.bank[0];
+        __half* packed = isv ? a.packed[1] : a.packed[0];
+        const int ld = isv ? a.ld[1] : a.ld[0], ldb = isv ? a.ldb[1] : a.ldb[0];
+        const float4 v = __ldg(reinterpret_cast<const float4*>(src + (size_t)r * ld + j * 4));
+        if (bank) *reinterpret_cast<float4*>(bank + (size_t)(off + r) * ldb + j * 4) = v;
+        if (packed) {
+            const __half2 h0 = __floats2half2_rn(v.x, v.y), h1 = __floats2half2_rn(v.z, v.w);
+            const __half2 l0 = __floats2half2_rn(v.x - __low2float(h0), v.y - __high2float(h0));
+            const __half2 l1 = __floats2half2_rn(v.z - __low2float(h1), v.w - __high2float(h1));
+            __half* d = packed + ((size_t)(j >> 3) * cap_rows + off + r) * 64 + (j & 7) * 4;
+            uint2 hi, lo;
+            hi.x = *reinterpret_cast<const unsigned*>(&h0); hi.y = *reinterpret_cast<const unsigned*>(&h1);
+            lo.x = *reinterpret_cast<const unsigned*>(&l0); lo.y = *reinterpret_cast<const unsigned*>(&l1);
+            *reinterpret_cast<uint2*>(d) = hi;
+            *reinterpret_cast<uint2*>(d + 32) = lo;
+        }
+    }
+}
+
+// After a store of `rows` rows: one more frame is live until the bank is full; the write offset moves on by one frame and
+// wraps to the first unpinned row when the next frame would not fit.
+__global__ void ring_advance_kernel(int* live, int* write, int rows, int cap_rows, int pinned_rows) {
+    pdl_sync();
+    *live = min(*live + rows, cap_rows);
+    int w = *write + rows;
+    if (w + rows > cap_rows) w = pinned_rows;
+    *write = w;
+}
+
 }  // namespace aotb
 
 using namespace aotb;
@@ -407,4 +462,38 @@ extern "C" int aotb_counter_add(int* counter, int delta, void* stream) {
     AOTB_REQUIRE(counter, "aotb_counter_add: null");
     launch(counter_add_kernel, dim3(1), dim3(1), 0, (cudaStream_t)stream, counter, delta);
     return check_launch("aotb_counter_add");
+}
+
+extern "C" int aotb_bank_ring_store(const float* k_src, int ldk, int k_cols, const float* v_src, int ldv, int v_cols, int rows,
+                                    float* k_bank, int ldkb, float* v_bank, int ldvb, void* k_packed, void* v_packed,
+                                    int cap_rows, const int* write, void* stream) {
+    AOTB_REQUIRE(k_src && v_src && write && rows > 0 && rows <= cap_rows, "aotb_bank_ring_store: bad args");
+    AOTB_REQUIRE(k_bank || v_bank || k_packed || v_packed, "aotb_bank_ring_store: no destination");
+    AOTB_REQUIRE(k_cols > 0 && v_cols > 0 && k_cols % 4 == 0 && v_cols % 4 == 0 && ldk % 4 == 0 && ldv % 4 == 0 &&
+                 ldk >= k_cols && ldv >= v_cols, "aotb_bank_ring_store: columns and row strides must be multiples of 4");
+    AOTB_REQUIRE((!k_bank || (ldkb % 4 == 0 && ldkb >= k_cols)) && (!v_bank || (ldvb % 4 == 0 && ldvb >= v_cols)),
+                 "aotb_bank_ring_store: bank row stride");
+    AOTB_REQUIRE((!k_packed || k_cols % 32 == 0) && (!v_packed || v_cols % 32 == 0),
+                 "aotb_bank_ring_store: a packed copy needs a multiple of 32 channels");
+    AOTB_REQUIRE(((uintptr_t)k_src | (uintptr_t)v_src | (uintptr_t)k_bank | (uintptr_t)v_bank | (uintptr_t)k_packed |
+                  (uintptr_t)v_packed) % 16 == 0, "aotb_bank_ring_store: alignment");
+    RingStoreArgs a;
+    a.src[0] = k_src; a.src[1] = v_src; a.bank[0] = k_bank; a.bank[1] = v_bank;
+    a.packed[0] = (__half*)k_packed; a.packed[1] = (__half*)v_packed;
+    a.ld[0] = ldk; a.ld[1] = ldv; a.ldb[0] = ldkb; a.ldb[1] = ldvb; a.c4[0] = k_cols / 4; a.c4[1] = v_cols / 4;
+    const size_t total = (size_t)rows * (a.c4[0] + a.c4[1]);
+    int g = (int)((total + 255) / 256);
+    if (g > 132 * 8) g = 132 * 8;
+    launch(bank_ring_store_kernel, dim3(g), dim3(256), 0, (cudaStream_t)stream, a, rows, cap_rows, write);
+    return check_launch("aotb_bank_ring_store");
+}
+
+extern "C" int aotb_ring_advance(int* live, int* write, int rows, int cap_rows, int pinned_rows, void* stream) {
+    AOTB_REQUIRE(live && write, "aotb_ring_advance: null counter");
+    AOTB_REQUIRE(rows > 0 && pinned_rows >= 0 && (long long)pinned_rows + rows <= cap_rows &&
+                 (cap_rows - pinned_rows) % rows == 0,
+                 "aotb_ring_advance: need rows > 0, pinned_rows + rows <= cap_rows and (cap_rows - pinned_rows) %% rows == 0 "
+                 "(got rows %d, cap_rows %d, pinned_rows %d)", rows, cap_rows, pinned_rows);
+    launch(ring_advance_kernel, dim3(1), dim3(1), 0, (cudaStream_t)stream, live, write, rows, cap_rows, pinned_rows);
+    return check_launch("aotb_ring_advance");
 }

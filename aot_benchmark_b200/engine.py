@@ -7,7 +7,8 @@ and tools/demo.py drive it unedited.  Differences are internal:
 
 * activations live in NHWC / token-major fp32 buffers allocated once per video;
 * the long-term memory is a pre-allocated append buffer (bank) instead of torch.cat'ed tensors
-  (new frames are appended, not prepended -- attention is permutation invariant over keys);
+  (new frames are appended, not prepended -- attention is permutation invariant over keys); with long_term_mem_max = M it
+  holds the first memory frame and the newest M - 1 in a ring, so a long clip runs at constant cost;
 * every FLOP of the per-frame path runs in libaotb200.so; there is no eager fallback and the
   engines refuse CPU tensors.
 
@@ -94,6 +95,16 @@ def _apply_pdl():
     lib().aotb_set_pdl(1 if USE_PDL else 0)
     check(lib().aotb_set_conv_tiling(_CONV_TILING_MASK[CONV_TILING]), "aotb_set_conv_tiling")
 BANK_INIT_FRAMES = int(_os.environ.get("AOTB_BANK_FRAMES", "24"))   # initial long-term bank capacity (memory frames)
+
+
+def _resolve_mem_max(aot_model, long_term_mem_max):
+    """The bound M of the long-term bank in memory frames: the keyword, else cfg.TEST_LONG_TERM_MEM_MAX, else None (unbounded)."""
+    m = getattr(aot_model.cfg, "TEST_LONG_TERM_MEM_MAX", None) if long_term_mem_max is None else long_term_mem_max
+    if m is None:
+        return None
+    if int(m) != m or m < 2:
+        raise ValueError(f"long_term_mem_max must be an integer >= 2 (the first memory frame and at least one recent one), got {m}")
+    return int(m)
 
 
 REPLAYED_KERNELS = [0]      # kernels launched through graph replays (bench.py adds this to the library's eager count)
@@ -477,7 +488,10 @@ class _Encoder:
 # single engine (<= max_obj_num objects)
 # =====================================================================================
 class AOTEngine(nn.Module):
-    def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1):
+    def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1, long_term_mem_max=None):
+        """long_term_mem_max = M bounds the long-term bank to M memory frames: the first frame stored after
+        restart_engine() stays, the other M - 1 slots hold the newest stored frames (the oldest is overwritten).  None: the
+        bound of cfg.TEST_LONG_TERM_MEM_MAX if the config has one, else the reference's ever-growing memory."""
         super().__init__()
         self.cfg = aot_model.cfg
         self.align_corners = aot_model.cfg.MODEL_ALIGN_CORNERS
@@ -486,6 +500,7 @@ class AOTEngine(nn.Module):
         self.gpu_id = gpu_id
         self.long_term_mem_gap = long_term_mem_gap
         self.short_term_mem_skip = short_term_mem_skip
+        self.long_term_mem_max = _resolve_mem_max(aot_model, long_term_mem_max)
         self.losses = None
         self._enc = None
         self._ws = None
@@ -493,6 +508,7 @@ class AOTEngine(nn.Module):
         self._P = None
         self.graphs = GraphCache()
         self.tk_dev = None
+        self.wr_dev = None            # bounded bank: row offset of the next stored memory frame
         self.kv_shard = None          # (rank, world, process_group) when the long-term bank is sharded over GPUs
         self.restart_engine()
 
@@ -523,6 +539,7 @@ class AOTEngine(nn.Module):
         self._mem_frames = 0          # memory frames stored so far (global count, all shards)
         if self.tk_dev is not None:
             self.tk_dev.zero_()
+            self.wr_dev.zero_()
 
     def enable_kv_sharding(self, rank, world, group=None):
         """BASELINE config 4: shard the long-term bank by memory frame round-robin over `world` ranks.  Every rank
@@ -531,6 +548,9 @@ class AOTEngine(nn.Module):
         (one NCCL collective per layer) and merged exactly (log-sum-exp) on every rank."""
         if not (LT_IMPL.startswith("tc") and not self._plan_is_deaot()):
             raise NotImplementedError("sharded long-term attention is implemented for the AOT tensor-core kernel")
+        if self.long_term_mem_max is not None:
+            raise NotImplementedError("a bounded long-term bank (long_term_mem_max) cannot be sharded over GPUs: each rank "
+                                      "would need its own ring")
         self.kv_shard = (int(rank), int(world), group)
 
     def _plan_is_deaot(self):
@@ -554,16 +574,22 @@ class AOTEngine(nn.Module):
         N = self.enc_hw
         C = P.C
         L = P.L
-        key = (id(P), N, tuple(self.enc_size_2d), tuple(self.input_size_2d), LT_IMPL, DEAOT_LT)
+        M = self.long_term_mem_max
+        if M is not None and P.deaot and DEAOT_LT == "gemm":
+            raise NotImplementedError("a bounded long-term bank (long_term_mem_max) is not built for AOTB_DEAOT_LT=gemm: its "
+                                      "transposed value copies have no ring store; use the default fused kernel")
+        key = (id(P), N, tuple(self.enc_size_2d), tuple(self.input_size_2d), LT_IMPL, DEAOT_LT, M)
         if self._ws is not None and self._ws_key == key:
             # same geometry and weights as the previous video: keep buffers and captured graphs
             self.bank_len = 0
             self.tk_dev.zero_()
+            self.wr_dev.zero_()
             self._st_ring = []
             return
         self._ws_key = key
         self.graphs.clear()
         self.tk_dev = torch.zeros(1, dtype=torch.int32, device=dev)    # live rows of the long-term bank
+        self.wr_dev = torch.zeros(1, dtype=torch.int32, device=dev)
         f = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
         ws = type("WS", (), {})()
         ws.N = N
@@ -609,6 +635,8 @@ class AOTEngine(nn.Module):
         ws.mask = f(*self.input_size_2d)                            # static copy of the caller's label map
         self._dec_out = {}
         cap = (min(BANK_INIT_FRAMES, GEMM_GROW_FRAMES) if (P.deaot and DEAOT_LT == "gemm") else BANK_INIT_FRAMES) * N
+        if M is not None:
+            cap = M * N               # bounded: allocated once, slot s = rows [s N, (s + 1) N), never re-allocated
         self.bank_cap = cap
         self.bank_K = [f(cap, self._kdim) for _ in range(L)]
         self.bank_V = [f(cap, self._vdim) for _ in range(L)]
@@ -660,7 +688,7 @@ class AOTEngine(nn.Module):
         (self._ws if ws is None else ws).S = torch.empty((self.enc_hw, capw), dtype=torch.float32, device=dev)
 
     def _bank_reserve(self, rows):
-        if self.bank_len + rows <= self.bank_cap:
+        if self.bank_len + rows <= self.bank_cap or self.long_term_mem_max is not None:
             return
         new_cap = max(2 * self.bank_cap, self.bank_len + rows)
         if getattr(self, "_gemm_lt", False):
@@ -692,6 +720,9 @@ class AOTEngine(nn.Module):
     # ------------------------------------------------------------------ reference-shaped views
     @property
     def long_term_memories(self):
+        """The live rows of the bank, per layer, in the reference's list-of-lists shape.  Rows are in storage order: the order
+        the frames were stored in for the unbounded bank; with long_term_mem_max = M, slot order (slot 0 = the first frame,
+        slots 1 .. M - 1 the ring, which is not age order once it has wrapped)."""
         if self.bank_len == 0:
             return None
         P = self._plan()
@@ -803,7 +834,7 @@ class AOTEngine(nn.Module):
         if self._claim_memory_frame():
             self._bank_reserve(self.enc_hw)
             self._append_short_to_bank(st)
-            self.bank_len += self.enc_hw
+            self.bank_len = self._bank_len_after_store()
         self.last_mem_step = self.frame_step
         self._have_lstt = True
 
@@ -854,7 +885,12 @@ class AOTEngine(nn.Module):
             if append:
                 self._append_short_to_bank(st)
         if append:
-            self.bank_len += self.enc_hw
+            self.bank_len = self._bank_len_after_store()
+
+    def _bank_len_after_store(self):
+        """Host copy of the live row count: one more frame, saturating at the capacity of a bounded bank."""
+        n = self.bank_len + self.enc_hw
+        return n if self.long_term_mem_max is None else min(n, self.bank_cap)
 
     def _claim_memory_frame(self):
         """Count one more memory frame (global count, all shards) and say whether THIS rank stores it: always without
@@ -868,6 +904,15 @@ class AOTEngine(nn.Module):
         host-side row count and capacity are the caller's business, so the body can be captured in a graph)."""
         N = self.enc_hw
         K_src, V_src = self._latest_kv()
+        if self.long_term_mem_max is not None:
+            # bounded: one launch per layer writes the fp32 rows and the packed rows of the selected attention kernel at the
+            # ring's write offset, then both counters move (the first frame's slot is never the wrap target)
+            packed = (self.bank_Kp, self.bank_Vp) if self._tc else (self.bank_gpK, self.bank_gpV) if self._gp_tc else None
+            for li in range(self._plan().L):
+                ops.bank_ring_store(K_src[li], V_src[li], self.bank_K[li], self.bank_V[li],
+                                    packed[0][li] if packed else None, packed[1][li] if packed else None, self.wr_dev, stream=st)
+            ops.ring_advance(self.tk_dev, self.wr_dev, N, self.bank_cap, N, stream=st)
+            return
         off = self.tk_dev
         for li in range(self._plan().L):
             ops.bank_append(K_src[li], self.bank_K[li], 0, offset_dev=off, stream=st)
@@ -1190,8 +1235,8 @@ class DeAOTEngine(AOTEngine):
     """networks/engines/deaot_engine.py:9-56 -- GatedPropagationModule stack (transformer.py:501-665)."""
 
     def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1,
-                 layer_loss_scaling_ratio=2.):
-        super().__init__(aot_model, gpu_id, long_term_mem_gap, short_term_mem_skip)
+                 layer_loss_scaling_ratio=2., long_term_mem_max=None):
+        super().__init__(aot_model, gpu_id, long_term_mem_gap, short_term_mem_skip, long_term_mem_max=long_term_mem_max)
         self.layer_loss_scaling_ratio = layer_loss_scaling_ratio
 
     def _gated_tail(self, core, U, dw_w, out_slice, h, w, st):
@@ -1345,7 +1390,9 @@ class DeAOTEngine(AOTEngine):
 class AOTInferEngine(nn.Module):
     _engine_cls = AOTEngine
 
-    def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1, max_aot_obj_num=None):
+    def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1, max_aot_obj_num=None,
+                 long_term_mem_max=None):
+        """long_term_mem_max: bound of every sub-engine's long-term bank in memory frames (see AOTEngine)."""
         super().__init__()
         self.cfg = aot_model.cfg
         self.AOT = aot_model
@@ -1356,12 +1403,16 @@ class AOTInferEngine(nn.Module):
         self.gpu_id = gpu_id
         self.long_term_mem_gap = long_term_mem_gap
         self.short_term_mem_skip = short_term_mem_skip
+        self.long_term_mem_max = _resolve_mem_max(aot_model, long_term_mem_max)
         self.aot_engines = []
         self._kv_shard = None
         self.restart_engine()
 
     def enable_kv_sharding(self, rank, world, group=None):
         """Shard the long-term memory bank over `world` ranks (see AOTEngine.enable_kv_sharding)."""
+        if self.long_term_mem_max is not None:
+            raise NotImplementedError("a bounded long-term bank (long_term_mem_max) cannot be sharded over GPUs: each rank "
+                                      "would need its own ring")
         self._kv_shard = (rank, world, group)
         for e in self.aot_engines:
             e.enable_kv_sharding(rank, world, group)
@@ -1446,7 +1497,9 @@ class AOTInferEngine(nn.Module):
         want = max(-(-int(obj_nums) // self.max_aot_obj_num), 1)          # ceil(objects / max_aot_obj_num), at least one
         while len(self.aot_engines) < want:
             eng = self._pool.pop(0) if self._pool else self._engine_cls(self.AOT, self.gpu_id, self.long_term_mem_gap,
-                                                                       self.short_term_mem_skip)
+                                                                       self.short_term_mem_skip,
+                                                                       long_term_mem_max=self.long_term_mem_max)
+            eng.long_term_mem_max = self.long_term_mem_max      # pooled engines too: part of their workspace key
             eng.restart_engine()
             eng.eval()
             if self._kv_shard is not None:

@@ -714,6 +714,47 @@ def counter_add(counter, delta, stream=None):
     return counter
 
 
+def _counter(name, c):
+    if c is None or not c.is_cuda or c.dtype != torch.int32 or c.numel() != 1:
+        raise AotbError(f"{name} must be an int32 CUDA tensor [1]")
+    return c.data_ptr()
+
+
+def bank_ring_store(k_src, v_src, k_bank, v_bank, k_packed, v_packed, write_dev, stream=None):
+    """Bounded bank: store one memory frame's k_src [rows, Ck] / v_src [rows, Cv] at row `*write_dev` of every copy given:
+    the fp32 banks k_bank [cap, >= Ck] / v_bank [cap, >= Cv] and the packed fp16 banks k_packed [Ck/32, cap, 64] / v_packed
+    [Cv/32, cap, 64] (the rows tc_pack_rows writes); a copy that is None is skipped.  All copies share one capacity."""
+    _chk(k_src, v_src, k_bank, v_bank)
+    if k_src.dim() != 2 or v_src.dim() != 2 or k_src.shape[0] != v_src.shape[0]:
+        raise AotbError("bank_ring_store: k_src and v_src must be [rows, C] with the same rows")
+    rows = k_src.shape[0]
+    caps = set()
+    for name, src, bank, packed in (("k", k_src, k_bank, k_packed), ("v", v_src, v_bank, v_packed)):
+        cols = src.shape[1]
+        if bank is not None:
+            if bank.dim() != 2 or bank.shape[1] < cols:
+                raise AotbError(f"bank_ring_store: {name}_bank {tuple(bank.shape)} is narrower than the {cols} source channels")
+            caps.add(bank.shape[0])
+        if packed is not None:
+            if packed.dtype != torch.float16 or not packed.is_cuda or not packed.is_contiguous() or packed.dim() != 3 or \
+                    packed.shape[2] != 64 or packed.shape[0] * 32 != cols:
+                raise AotbError(f"bank_ring_store: {name}_packed must be a contiguous fp16 CUDA tensor [{cols} / 32, cap, 64]")
+            caps.add(packed.shape[1])
+    if len(caps) != 1 or rows > min(caps):
+        raise AotbError(f"bank_ring_store: the copies need one capacity of at least {rows} rows, got {sorted(caps)}")
+    check(lib().aotb_bank_ring_store(_p(k_src), k_src.stride(0), k_src.shape[1], _p(v_src), v_src.stride(0), v_src.shape[1],
+                                     rows, _p(k_bank), k_bank.stride(0) if k_bank is not None else 0, _p(v_bank),
+                                     v_bank.stride(0) if v_bank is not None else 0, _p(k_packed), _p(v_packed), caps.pop(),
+                                     _counter("bank_ring_store: write_dev", write_dev), _st(stream)), "aotb_bank_ring_store")
+
+
+def ring_advance(live_dev, write_dev, rows, cap_rows, pinned_rows, stream=None):
+    """Bounded bank, after a store of `rows` rows: *live_dev = min(*live_dev + rows, cap_rows); *write_dev moves on by `rows`
+    and wraps to `pinned_rows` when the next store would pass `cap_rows` (both int32 CUDA tensors [1])."""
+    check(lib().aotb_ring_advance(_counter("ring_advance: live_dev", live_dev), _counter("ring_advance: write_dev", write_dev),
+                                  int(rows), int(cap_rows), int(pinned_rows), _st(stream)), "aotb_ring_advance")
+
+
 # ------------------------------------------------------------------ tensor-core long-term attention
 def tc_pack_rows(src, dst, row_off=0, div=1.0, row_off_dev=None, stream=None):
     """src fp32 [rows, H*32] -> dst fp16 [H, cap, 64] rows [row_off, row_off+rows) as [hi(32) | lo(32)]."""

@@ -303,6 +303,25 @@ int aotb_bank_append_f32(const float* src, int lds, float* bank, int ldb, int ro
                          const int* offset_dev, void* stream);
 int aotb_counter_add(int* counter, int delta, void* stream);
 
+/* Bounded long-term bank: at most cap_rows / rows memory frames, the first one pinned in rows [0, pinned_rows), the others a
+ * FIFO ring over rows [pinned_rows, cap_rows).  Two device counters carry the state, so both calls can sit in a replayed graph:
+ * *live = rows the attention kernels read (their Tk_dev), *write = row offset of the next store.
+ *   aotb_bank_ring_store: ONE launch stores a memory frame's keys k_src [rows][ldk] (k_cols channels) and values v_src
+ *                         [rows][ldv] (v_cols channels) at row *write of every copy of the bank that is given: the fp32 banks
+ *                         k_bank / v_bank [cap_rows][ldkb / ldvb] (equal to the source) and the split-fp16 banks k_packed /
+ *                         v_packed [cols / 32][cap_rows][64] (bit for bit the rows aotb_tc_pack_rows_f16x2 writes with
+ *                         div = 1).  A null destination is skipped.  All pointers 16-byte aligned, columns and row strides
+ *                         multiples of 4, packed copies need multiples of 32 channels.  A store that does not fit
+ *                         (*write < 0 or *write + rows > cap_rows) writes nothing.
+ *   aotb_ring_advance   : after such a store, *live = min(*live + rows, cap_rows); *write += rows, and *write = pinned_rows
+ *                         if a further store of `rows` rows there would pass cap_rows.  Requires rows > 0,
+ *                         pinned_rows + rows <= cap_rows and (cap_rows - pinned_rows) % rows == 0, so starting from
+ *                         *write = 0 (with pinned_rows a multiple of rows) no store ever passes the end of the bank. */
+int aotb_bank_ring_store(const float* k_src, int ldk, int k_cols, const float* v_src, int ldv, int v_cols, int rows,
+                         float* k_bank, int ldkb, float* v_bank, int ldvb, void* k_packed, void* v_packed, int cap_rows,
+                         const int* write, void* stream);
+int aotb_ring_advance(int* live, int* write, int rows, int cap_rows, int pinned_rows, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
