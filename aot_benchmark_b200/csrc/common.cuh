@@ -105,8 +105,8 @@ __device__ __forceinline__ float apply_act(float v, int act) {
 
 // h_swish = v * h_sigmoid(v) (mobilenetv3.py:42-48) stays out of apply_act, so every kernel that existed before it compiles
 // exactly as before.  The kernels MobileNetV3 runs take it as a template flag (fp32 conv finish, depthwise conv: HS selects the
-// instantiation, so the existing ones are unchanged) or as a runtime code (gate scale, apply_act_hs); the tensor-core conv, the
-// conv chain and GroupNorm reject ACT_HSWISH at their entry points.
+// instantiation, so the existing ones are unchanged) or as a runtime code (gate scale, apply_act_hs); the tensor-core conv and
+// GroupNorm reject ACT_HSWISH at their entry points.
 template <bool HS>
 __device__ __forceinline__ float apply_act_or_hswish(float v, int act) {
     return HS ? v * hsigmoid(v) : apply_act(v, act);

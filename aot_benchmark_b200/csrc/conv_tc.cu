@@ -28,10 +28,31 @@
 // times at BN = 64.  STAGES: 4 at BN = 64, 3 at 128, 2 at 256 (a stage is 32 KB of A plus BN * 256 bytes of B).
 #include <type_traits>
 
-#include "conv_tc.cuh"
+#include "common.cuh"
+#include "tc_common.cuh"
 
 namespace aotb {
 namespace tc {
+
+constexpr int CONV_A_BYTES = 128 * 128;        // one 128 x 64 half tile (both consumer warpgroups' rows)
+
+template <int BN>
+__device__ __forceinline__ void wgmma_conv(float* acc, uint64_t a, uint64_t b) {
+    if (BN == 256) wgmma_ss_n256(acc, a, b, 1u);
+    else if (BN == 128) wgmma_ss_n128(acc, a, b, 1u);
+    else wgmma_ss_n64(acc, a, b, 1u);
+}
+
+// Accumulator fragment -> row-major fp32 staging tile [128][ld] (row = pixel of the tile, column = channel of the tile).
+template <int BN>
+__device__ __forceinline__ void conv_acc_to_staging(const float* acc, float* stg, int ld) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int row0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2), cq = (lane & 3) * 2;
+#pragma unroll
+    for (int j = 0; j < BN / 2; j += 2)
+        *reinterpret_cast<float2*>(stg + (row0 + 8 * ((j >> 1) & 1)) * ld + 8 * (j >> 2) + cq) = make_float2(acc[j], acc[j + 1]);
+}
+
 struct ConvTcArgs {
     const float* in;
     const float* bias;

@@ -233,8 +233,6 @@ class _Encoder:
     def _body(self, x):
         P = self.plan
         st = _cur_stream()
-        if P.encoder_name == "resnet50" and ops.CONV_CHAIN and ops.CONV_IMPL == "tc":
-            return self._resnet_chain(x, st)
         if P.encoder_name in ("resnet50", "resnet101"):
             feats = self._resnet(x, st)
         elif P.encoder_name in ("resnest50", "resnest101"):
@@ -329,49 +327,6 @@ class _Encoder:
                 cur, h, w = out, ho, wo
             feats.append(cur)
         return feats
-
-    def _resnet_chain(self, x, st):
-        """ResNet-50 stages + projector as ONE persistent dataflow kernel (ops.ConvChain, csrc/conv_chain.cu): the 7x7 stem and
-        the max-pool stay separate launches, the 52 bottleneck convs and the 1x1 projector become a tile program.  Every layer
-        output gets its own buffer (an address must not change twice inside one launch: the L1 caches are not coherent)."""
-        P = self.plan
-        e = P.enc
-        H, W = x.shape[1], x.shape[2]
-        h1, w1 = self._osz(H, 7, 2, 3), self._osz(W, 7, 2, 3)
-        c1 = self._buf("stem", (1, h1, w1, 64))
-        ops.conv2d(x, e.stem.w, e.stem.b, c1, KH=7, KW=7, stride=2, pad=3, act=A_RELU, stream=st)
-        h, w = self._osz(h1, 3, 2, 1), self._osz(w1, 3, 2, 1)
-        pool = self._buf("pool", (1, h, w, 64))
-        ops.maxpool3x3s2(c1, pool, stream=st)
-        key = (id(P), H, W)
-        ch = getattr(self, "_chain", None)
-        if ch is None or ch[0] != key:
-            layers, feats = [], []
-            cur, cur_i = pool, -1                      # tensor + index of the chain layer that produces it (-1: the pool)
-            for si, blocks in enumerate(e.stages):
-                for bi, b in enumerate(blocks):
-                    ho, wo = self._osz(h, 3, b.stride, 1), self._osz(w, 3, b.stride, 1)
-                    t1 = self._buf(f"c{si}b{bi}t1", (1, h, w, b.c1.cout))
-                    layers.append(dict(x=cur, w=b.c1.w, bias=b.c1.b, out=t1, act=A_RELU, in_layer=cur_i))
-                    i1 = len(layers) - 1
-                    t2 = self._buf(f"c{si}b{bi}t2", (1, ho, wo, b.c2.cout))
-                    layers.append(dict(x=t1, w=b.c2.w, bias=b.c2.b, out=t2, KH=3, stride=b.stride, pad=1, act=A_RELU, in_layer=i1))
-                    i2 = len(layers) - 1
-                    if b.down is not None:
-                        res = self._buf(f"c{si}ds", (1, ho, wo, b.down.cout))
-                        layers.append(dict(x=cur, w=b.down.w, bias=b.down.b, out=res, stride=b.stride, in_layer=cur_i))
-                        res_i = len(layers) - 1
-                    else:
-                        res, res_i = cur, cur_i
-                    out = self._buf(f"c{si}o{bi}", (1, ho, wo, b.c3.cout))
-                    layers.append(dict(x=t2, w=b.c3.w, bias=b.c3.b, out=out, res=res, act=A_RELU, in_layer=i2, res_layer=res_i))
-                    cur, cur_i, h, w = out, len(layers) - 1, ho, wo
-                feats.append(cur)
-            proj = self._buf("proj", (1, h, w, P.C))
-            layers.append(dict(x=cur, w=P.proj.w, bias=P.proj.b, out=proj, in_layer=cur_i))
-            ch = self._chain = (key, ops.ConvChain(layers, self.dev, stream=st), feats, proj)
-        ch[1].run(st)
-        return [ch[2][0], ch[2][1], ch[2][2], ch[3]]
 
     def _swin(self, x4, st):
         """SwinTransformer.forward (swin_transformer.py:684-716) for 'swin_base': tokens stay one [H*W, C] matrix per

@@ -122,86 +122,8 @@ def _pow2(e):
     return ((e + 127) << 23).to(torch.int32).view(torch.float32)
 
 
-# ---- a chain of tensor-core convs as one persistent dataflow kernel (csrc/conv_chain.cu)
-CONV_CHAIN = os.environ.get("AOTB_CONV_CHAIN", "0") == "1"
-
-
-def _chain_struct():
-    import ctypes
-
-    class ChainLayer(ctypes.Structure):
-        _fields_ = [(n, ctypes.c_void_p) for n in ("inp", "wh", "wl", "bias", "wscale", "res", "out")] + \
-                   [(n, ctypes.c_int) for n in ("H", "W", "Cin", "ldin", "Cout", "ldout", "ldres", "KH", "KW", "stride", "pad",
-                                                "act", "in_layer", "res_layer")]
-    return ChainLayer
-
-
-def conv_chain_layers(layers):
-    """layers: list of dicts (x [1,H,W,Cin] NHWC view, w fp32 [K, Cout] registered for the tensor-core path, bias, out, res,
-    KH, stride, pad, act, in_layer, res_layer) -> ctypes array of aotb_chain_layer (keeps the tensors alive via the dicts)."""
-    CL = _chain_struct()
-    arr = (CL * len(layers))()
-    for i, l in enumerate(layers):
-        x, out, res = l["x"], l["out"], l.get("res")
-        t = _TC_WEIGHTS.get(l["w"].data_ptr())
-        if t is None:
-            raise AotbError("conv_chain: layer weights are not registered for the tensor-core path")
-        _chk(x, l["bias"], out, res)
-        B, H, W, Cin = x.shape
-        if B != 1:
-            raise AotbError("conv_chain: batch 1 only")
-        a = arr[i]
-        a.inp, a.wh, a.wl = x.data_ptr(), t[0].data_ptr(), t[1].data_ptr()
-        a.bias, a.wscale, a.res, a.out = _p(l["bias"]), _p(t[2]), _p(res), out.data_ptr()
-        a.H, a.W, a.Cin, a.ldin = H, W, Cin, _nhwc_ld(x)
-        a.Cout, a.ldout, a.ldres = out.shape[3], _nhwc_ld(out), (_nhwc_ld(res) if res is not None else 0)
-        a.KH = a.KW = l.get("KH", 1)
-        a.stride, a.pad, a.act = l.get("stride", 1), l.get("pad", 0), l.get("act", ACT_NONE)
-        a.in_layer, a.res_layer = l.get("in_layer", -1), l.get("res_layer", -1)
-    return arr
-
-
-def conv_chain_dump(layers):
-    """Host-only: -> (work items [n, 8] = layer, m-tile, n-tile, dep_lo, dep_hi, k0, k1, split; layer table [L, 10] = M, BN,
-    counters offset, producer / residual counters offset (-1: none), in_need, res_need, splits, partial counters offset, chunks)."""
-    import ctypes
-    arr = layers if not isinstance(layers, list) else conv_chain_layers(layers)
-    n = len(arr)
-    nbytes, ntiles, ncnt = ctypes.c_size_t(), ctypes.c_int(), ctypes.c_int()
-    check(lib().aotb_conv_chain_plan(ctypes.addressof(arr), n, ctypes.addressof(nbytes), ctypes.addressof(ntiles),
-                                     ctypes.addressof(ncnt)), "aotb_conv_chain_plan")
-    tiles = (ctypes.c_int * (8 * ntiles.value))()
-    lay = (ctypes.c_int * (10 * n))()
-    check(lib().aotb_conv_chain_dump(ctypes.addressof(arr), n, ctypes.addressof(tiles), ntiles.value, ctypes.addressof(lay)),
-          "aotb_conv_chain_dump")
-    return [list(tiles[8 * i:8 * i + 8]) for i in range(ntiles.value)], [list(lay[10 * i:10 * i + 10]) for i in range(n)]
-
-
-class ConvChain:
-    """A built chain program: `run(stream)` clears the dependency counters and launches the persistent kernel."""
-
-    def __init__(self, layers, device, stream=None):
-        import ctypes
-        self.layers = layers                                   # keeps every tensor of the program alive
-        arr = conv_chain_layers(layers)
-        self.n = len(layers)
-        nbytes, ntiles, ncnt = ctypes.c_size_t(), ctypes.c_int(), ctypes.c_int()
-        check(lib().aotb_conv_chain_plan(ctypes.addressof(arr), self.n, ctypes.addressof(nbytes), ctypes.addressof(ntiles),
-                                         ctypes.addressof(ncnt)), "aotb_conv_chain_plan")
-        self.ntiles, self.ncounters = ntiles.value, ncnt.value
-        self.program = torch.zeros(nbytes.value + 256, dtype=torch.uint8, device=device)
-        self._base = (self.program.data_ptr() + 255) // 256 * 256
-        check(lib().aotb_conv_chain_build(ctypes.addressof(arr), self.n, self._base, nbytes.value, _st(stream)),
-              "aotb_conv_chain_build")
-
-    def run(self, stream=None):
-        check(lib().aotb_conv_chain_run(self._base, self.n, self.ntiles, self.ncounters, _st(stream)), "aotb_conv_chain_run")
-
-    def profile(self):
-        """AOTB_CHAIN_PROF=1: per work item [picked up, inputs complete, accumulator complete, published] in ns (globaltimer)."""
-        off = lib().aotb_conv_chain_prof_offset(self.n, self.ntiles, self.ncounters) + (self._base - self.program.data_ptr())
-        torch.cuda.synchronize()
-        return self.program[off:off + self.ntiles * 32].view(torch.int64).view(self.ntiles, 4).cpu()
+# bench.py's encoder probe saves this flag, sets it False and restores it; no encoder path reads it
+CONV_CHAIN = False
 
 
 def conv2d_tc(x, wh, wl, bias, out, res=None, KH=1, KW=1, stride=1, pad=0, act=ACT_NONE, stream=None, wscale=None):

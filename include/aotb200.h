@@ -43,7 +43,7 @@ int aotb_set_conv_tiling(int mode);
  * in [B][H][W][ldin], w [KH*KW*Cin][Cout], out [B][Ho][Wo][ldout], res like out with ldres.
  * act: 0 none, 1 ReLU, 2 exact GELU, 3 SiLU, 4 ReLU6, 5 h_swish = v * relu6(v + 3) / 6 (networks/encoders/mobilenetv3.py:33-48,
  * true division by 6).  h_swish is taken by this conv, aotb_linear_f32, aotb_dwconv_nhwc_f32 and aotb_gate_scale_f32; the
- * tensor-core conv, the conv chain and GroupNorm accept 0-4 only. */
+ * tensor-core conv and GroupNorm accept 0-4 only. */
 int aotb_conv2d_nhwc_f32(const float* in, const float* w, const float* bias, const float* res, float* out,
                          int B, int H, int W, int Cin, int ldin, int Cout, int ldout, int ldres,
                          int KH, int KW, int stride, int pad, int dil, int act, void* stream);
@@ -213,32 +213,6 @@ int aotb_soft_logit_aggregation_f32(const float* const* logits, int n_engines, i
 /* networks/engines/aot_engine.py:515-533 (AOTInferEngine.separate_mask, label-map form): out[e][i] = mask[i] - e*max_obj if
  * e*max_obj < mask[i] <= (e+1)*max_obj else 0, for e in [0, n_engines). */
 int aotb_separate_labels_f32(const float* mask, int n_engines, int max_obj, float* out, int HW, void* stream);
-/* A chain of tensor-core convolutions as ONE persistent kernel with tile-level dataflow (csrc/conv_chain.cu): replaces the
- * per-layer launches of networks/encoders/resnet.py:34-54,140-157 (Bottleneck stacks, FrozenBN folded) by a program of 128-pixel
- * tiles that start as soon as the tiles of the producing layer they read are complete.  Every layer follows the contract of
- * aotb_conv2d_nhwc_tc (fp32 NHWC in / out, pre-split fp16 weights [Cout][KH*KW*Cin], bias, optional residual, activation) with
- * Cin % 64 == 0 and Cout % 64 == 0; in_layer / res_layer name the chain layer that produces `in` / `res` (-1: complete before
- * the launch).  Every output buffer must be written by exactly one layer of the chain (the SMs' L1 caches are not coherent:
- * no address may change its value twice inside one launch).  aotb_conv_chain_plan sizes the device-resident program,
- * aotb_conv_chain_build writes it (once per geometry, outside stream capture), aotb_conv_chain_run clears the dependency
- * counters and launches the kernel (capturable); aotb_conv_chain_dump exposes the tile program to host-side tests.  Layers with
- * few tiles and a long K loop are cut into up to 4 split-K work items; the item that holds the last K range adds the others'
- * partial tiles (kept in a scratch area of the program buffer) in split order, so results are deterministic. */
-typedef struct aotb_chain_layer {
-    const float* in;
-    const void* wh;
-    const void* wl;
-    const float* bias;
-    const float* wscale;      /* per-output-channel factor of the finished sum, as in aotb_conv2d_nhwc_tc (NULL = 1) */
-    const float* res;
-    float* out;
-    int H, W, Cin, ldin, Cout, ldout, ldres, KH, KW, stride, pad, act, in_layer, res_layer;
-} aotb_chain_layer;
-int aotb_conv_chain_plan(const void* layers, int nlayers, size_t* program_bytes, int* ntiles, int* ncounters);
-int aotb_conv_chain_dump(const void* layers, int nlayers, int* tiles8, int max_tiles, int* layers10);
-int aotb_conv_chain_build(const void* layers, int nlayers, void* program, size_t program_bytes, void* stream);
-int aotb_conv_chain_run(void* program, int nlayers, int ntiles, int ncounters, void* stream);
-size_t aotb_conv_chain_prof_offset(int nlayers, int ntiles, int ncounters);
 /* Frame input side (SURVEY 8 f.3): dataloaders/eval_datasets.py:60-61 + dataloaders/video_transforms.py:594-715 (MultiRestrictSize's
  * cv2.resize(INTER_CUBIC) of the float image, MultiToTensor's / 255, - mean, / std, HWC -> CHW) on the uint8 frame in one pass.
  * img uint8 [H][W][3]; ix / cx [Wo][4] and iy / cy [Ho][4] = clamped tap indices and Keys-cubic (A = -0.75) weights per output

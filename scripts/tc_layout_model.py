@@ -1,4 +1,4 @@
-"""Address-level model of the Hopper tensor-core data path of csrc/attn_tc.cuh and csrc/conv_tc.cuh, in numpy.
+"""Address-level model of the Hopper tensor-core data path of csrc/attn_tc.cuh and csrc/conv_tc.cu, in numpy.
 
 Shared memory is a byte array.  TMA with SWIZZLE_128B stores row r of a [rows][64 halfs] tile at r * 128 with its 16-byte
 chunk c at chunk c ^ (r % 8); the conv producer writes its activation slots with the same formula as the kernel (soff).
@@ -138,17 +138,17 @@ def model_attention(Q, K, V, T, qc=1, bk=64):
 
 
 def model_conv_a_tile(X):
-    """conv_tc.cuh: thread (wg, q = t & 15, rsub = t >> 4) stores rows wg*64 + i*8 + rsub, 16-byte segment q, hi half at
-    soff + i*1024; the warpgroup's wgmma reads rows [wg*64, +64) K-major from start + wg*8192 + 32 ks.  X: [128][64] fp32
-    -> the [128][64] matrix (hi halves) the MMAs see."""
+    """conv_tc.cu: for half chunk `part`, producer thread p (q = p & 15, rsub = p >> 4) stores rows part*64 + i*8 + rsub,
+    16-byte segment q, hi half at soff + part*8192 + i*1024; consumer warpgroup wg's wgmma reads rows [wg*64, +64) K-major
+    from start + wg*8192 + 32 ks.  X: [128][64] fp32 -> the [128][64] matrix (hi halves) the MMAs see."""
     buf = np.zeros(128 * 128, np.uint8)
     hi = X.astype(np.float16)
-    for wg in range(2):
-        for t in range(128):
-            q, rsub = t & 15, t >> 4
-            soff = (wg * 64 + rsub) * 128 + (((q >> 1) ^ rsub) << 4) + ((q & 1) << 3)
+    for part in range(2):
+        for p in range(128):
+            q, rsub = p & 15, p >> 4
+            soff = (part * 64 + rsub) * 128 + (((q >> 1) ^ rsub) << 4) + ((q & 1) << 3)
             for i in range(8):
-                row = wg * 64 + i * 8 + rsub
+                row = part * 64 + i * 8 + rsub
                 buf[soff + i * 1024: soff + i * 1024 + 8] = hi[row, 4 * q:4 * q + 4].view(np.uint8)
     out = np.zeros((128, 64), np.float32)
     for wg in range(2):

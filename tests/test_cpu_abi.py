@@ -102,7 +102,7 @@ def test_every_ops_attribute_used_by_the_engine_exists():
     import ast
     from aot_benchmark_b200 import engine, ops
     for path, aliases in ((os.path.join(REPO, "aot_benchmark_b200", "engine.py"), {"ops": ops}),
-                          (os.path.join(REPO, "bench.py"), {"ops": ops, "engine_mod": engine}),
+                          (os.path.join(REPO, "bench.py"), {"ops": ops, "ops_mod": ops, "engine_mod": engine}),
                           (os.path.join(REPO, "__graft_entry__.py"), {})):
         tree = ast.parse(open(path).read())
         for node in ast.walk(tree):
@@ -131,7 +131,7 @@ def test_kernel_register_budgets_fit_their_block_sizes():
     r = subprocess.run(["cuobjdump", "-res-usage", _lib.LIB_PATH], capture_output=True, text=True)
     if r.returncode != 0:
         pytest.skip("cuobjdump unavailable")
-    blocks = {"attn_tc_kernel": 288, "conv_tc_kernel": 288, "conv_chain_kernel": 288, "local_attn_tile_kernel": 512,
+    blocks = {"attn_tc_kernel": 288, "conv_tc_kernel": 288, "local_attn_tile_kernel": 512,
               "conv_igemm_kernel": 256, "attn_f32_kernel": 256, "local_attn_kernel": 256, "window_attn_kernel": 64}
     cur, seen = None, 0
     for line in r.stdout.splitlines():

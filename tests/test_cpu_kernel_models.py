@@ -1,4 +1,4 @@
-"""CPU: GPU-free models of the tensor-core attention kernel (csrc/attn_tc.cuh) and the conv K loop (csrc/conv_tc.cuh):
+"""CPU: GPU-free models of the tensor-core attention kernel (csrc/attn_tc.cuh) and the conv K loop (csrc/conv_tc.cu):
   * a discrete-event model of the TMA / mbarrier K-V stage ring (parity waits, asynchronous wgmma reads) in the default and
     the "ahead" issue order and with the DeAOT kernel's parameters: no deadlock, no overwrite of a stage being read;
   * an address-level model of the data path (128B-swizzled tiles, wgmma descriptor offsets, accumulator and register

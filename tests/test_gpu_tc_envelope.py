@@ -2,7 +2,7 @@
 
 - Weight scale: the split-fp16 conv / linear with weights scaled by 2^k, and with channels whose rms spans 1e-4 .. 1e-1
   (FrozenBN folding makes such channels), stays within the fp32-accumulation bound in every channel, through the
-  per-layer kernel, ops.conv2d / ops.linear with registered weights, and the persistent conv chain.
+  per-layer kernel and ops.conv2d / ops.linear with registered weights.
 - Tiling: every N tile x split-K cluster size the conv kernel can be forced to, at M / K tails, general Cin, stride 2,
   batch 2, strided rows, an aliased residual and every activation.
 - Attention: the fused long-term attention kernels (all layouts, exact and fast) at the 64 / 128 tile edges, with a
@@ -131,56 +131,6 @@ def test_small_weight_channels(kind):
     finally:
         ops._TC_WEIGHTS.pop(wk.data_ptr(), None)
     assert torch.equal(out, out2)
-
-
-def test_conv_chain_small_weight_layers():
-    """A conv chain with small-weight layers, one of them split along K: each is within 1e-5 of every channel's max |ref|
-    (the scale is applied to the finished sum, never to the raw partials), and every layer not split along K stays
-    bit-identical to the per-layer kernel without split-K."""
-    from aot_benchmark_b200 import ops
-    from aot_benchmark_b200._lib import lib
-    g = torch.Generator().manual_seed(4)
-    layers, w4s = [], []
-
-    def conv(x, cout, k, w4, act):
-        pad = k // 2
-        wk = _pack_w(w4).to(DEV)
-        ops.register_tc_weights(wk, *ops.split_fp16_scaled(wk))
-        out = torch.full((1, x.shape[1], x.shape[2], cout), float("nan"), device=DEV)
-        layers.append(dict(x=x, w=wk, bias=(torch.randn(cout, generator=g) * 1e-3).to(DEV), out=out, KH=k, pad=pad, act=act,
-                           in_layer=len(layers) - 1))
-        w4s.append(w4)
-        return out
-
-    x0 = torch.randn(1, 23, 29, 64, generator=g).to(DEV)
-    t = conv(x0, 64, 1, torch.randn(64, 64, 1, 1, generator=g) / 8, 1)
-    t = conv(t, 128, 3, _mixed_weights(128, 64, 3, g), 0)        # small weights, 9 chunks: not split
-    t = conv(t, 128, 3, _mixed_weights(128, 128, 3, g), 0)       # small weights, 18 chunks: split along K
-    conv(t, 64, 1, torch.randn(64, 128, 1, 1, generator=g) / 11, 0)
-    try:
-        _, table = ops.conv_chain_dump(layers)
-        assert [r[7] for r in table] == [1, 1, 2, 1], table
-        chain = ops.ConvChain(layers, DEV)
-        chain.run()
-        torch.cuda.synchronize()
-        got = [l["out"].clone() for l in layers]
-        for i in (1, 2):
-            ref = _ref_conv(layers[i]["x"].cpu(), w4s[i], layers[i]["bias"].cpu(), 1, 1)
-            d, s = _channel_err(got[i], ref)
-            assert (d / s).max().item() < 1e-5, f"small-weight chain layer {i}: {(d / s).max().item():.2e}"
-        assert lib().aotb_set_conv_tiling(1 << 8) == 0                  # per-layer kernel without split-K
-        try:
-            for i, l in enumerate(layers):
-                one = torch.full_like(l["out"], float("nan"))
-                ops.conv2d(l["x"], l["w"], l["bias"], one, KH=l["KH"], KW=l["KH"], pad=l["pad"], act=l["act"])
-                torch.cuda.synchronize()
-                if table[i][7] == 1:
-                    assert torch.equal(got[i], one), f"layer {i}: max |d| = {(got[i] - one).abs().max().item():.3e}"
-        finally:
-            lib().aotb_set_conv_tiling(0)
-    finally:
-        for l in layers:
-            ops._TC_WEIGHTS.pop(l["w"].data_ptr(), None)
 
 
 # B, H, W, Cin, Cout, K, stride, pad, residual ("" | "res" | "alias"), act, wide (ldin / ldout / ldres wider than C)
