@@ -60,6 +60,11 @@ class EngineConfig:
         self.TRAIN_LONG_TERM_MEM_GAP = 2 if gap == 5 else 9999
         self.TEST_LONG_TERM_MEM_GAP = gap
         self.TEST_SHORT_TERM_MEM_SKIP = 1
+        # test-time augmentation and the frame size rule (configs/default.py:97-100); TTAInferEngine defaults to the first two
+        self.TEST_FLIP = False
+        self.TEST_MULTISCALE = [1]
+        self.TEST_MAX_SHORT_EDGE = None
+        self.TEST_MAX_LONG_EDGE = 800 * 1.3
         # keys the reference model constructors read (all inactive in eval)
         self.TRAIN_ENCODER_FREEZE_AT = 2
         self.TRAIN_LSTT_EMB_DROPOUT = 0.

@@ -231,6 +231,109 @@ __global__ void nearest_kernel(const float* __restrict__ in, float* __restrict__
     }
 }
 
+// Test-time augmentation (networks/managers/evaluator.py:265-446 with TEST_FLIP / TEST_MULTISCALE): E augmentations, each an
+// engine on its own resized and possibly mirrored copy of the frame.  Both kernels sample an augmentation's logit map with the
+// bilinear arithmetic of logits_argmax_kernel; a map already at the output size is read unchanged (bl_src gives weights 1 and
+// 0 there for either align_corners).
+struct TTAArgs {
+    const float* logits[8];     // [NC][h][w] per augmentation
+    int h[8], w[8];
+    int flip[8];
+};
+
+__device__ __forceinline__ float tta_sample(const float* __restrict__ b, int w, int y0, int y1, int x0, int x1, float ly,
+                                            float lx) {
+    const float hy = 1.f - ly, hx = 1.f - lx;
+    return hy * (hx * b[y0 * w + x0] + lx * b[y0 * w + x1]) + ly * (hx * b[y1 * w + x0] + lx * b[y1 * w + x1]);
+}
+
+// evaluator.py:332-361: per output pixel, every augmentation's upsampled logits (read at the mirrored column for a flipped
+// one, :336-337) -> softmax over NC (:339) -> mean over the augmentations in order (:355-358) -> first argmax (:359-361),
+// then the new-object overlay n != 0 ? n : label (:363-369).  The mean probabilities go to prob [NC][H][W] when it is given.
+// Three passes over the channels per augmentation (max, sum, probability): the E x NC logits stay in L1 / L2, nothing but the
+// label (and the optional probabilities) is written.
+__global__ void tta_merge_kernel(const TTAArgs a, int E, int NC, int Ho, int Wo, int align,
+                                 const float* __restrict__ new_label, float* __restrict__ label, float* __restrict__ prob) {
+    pdl_sync();
+    const int total = Ho * Wo;
+    const float inv_e = 1.f / (float)E;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+        const int oy = i / Wo, ox = i - oy * Wo;
+        int y0[8], y1[8], x0[8], x1[8];
+        float ly[8], lx[8], m[8], s[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            if (e < E) {
+                bl_src(oy, a.h[e], Ho, align, y0[e], y1[e], ly[e]);
+                bl_src(a.flip[e] ? Wo - 1 - ox : ox, a.w[e], Wo, align, x0[e], x1[e], lx[e]);
+                const size_t plane = (size_t)a.h[e] * a.w[e];
+                float mx = -INFINITY;
+                for (int c = 0; c < NC; ++c)
+                    mx = fmaxf(mx, tta_sample(a.logits[e] + c * plane, a.w[e], y0[e], y1[e], x0[e], x1[e], ly[e], lx[e]));
+                float sum = 0.f;
+                for (int c = 0; c < NC; ++c)
+                    sum += expf(tta_sample(a.logits[e] + c * plane, a.w[e], y0[e], y1[e], x0[e], x1[e], ly[e], lx[e]) - mx);
+                m[e] = mx;
+                s[e] = sum;
+            }
+        }
+        float best = -INFINITY;
+        int bi = 0;
+        for (int c = 0; c < NC; ++c) {
+            float acc = 0.f;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                if (e < E) {
+                    const float* b = a.logits[e] + c * (size_t)a.h[e] * a.w[e];
+                    acc += expf(tta_sample(b, a.w[e], y0[e], y1[e], x0[e], x1[e], ly[e], lx[e]) - m[e]) / s[e];
+                }
+            }
+            const float p = acc * inv_e;
+            if (prob) prob[(size_t)c * total + i] = p;
+            if (p > best) { best = p; bi = c; }
+        }
+        const float n = new_label ? new_label[i] : 0.f;
+        label[i] = n != 0.f ? n : (float)bi;
+    }
+}
+
+// evaluator.py:346-353, :363-422 for one augmentation: the label its engine stores in memory.  For input pixel (y, x) the
+// nearest source (sy, sx) at the output size follows nearest_kernel; base = argmax softmax of the upsampled logits at (sy, sx)
+// in the augmentation's own orientation (the flip of :336-337 and the flip back of :373-376 / :402-406 cancel), n = the
+// new-object label at the mirrored column for a flipped augmentation (mirror at output size first, then nearest: the two do not
+// commute), out = n != 0 ? n : base.  No logits: base = 0 (the first frame's label, :315-319); no new label: n = 0.
+__global__ void tta_feedback_kernel(const float* __restrict__ lo, int h, int w, int NC, int H, int W, int align, int flip,
+                                    const float* __restrict__ new_label, float* __restrict__ out, int Hi, int Wi) {
+    pdl_sync();
+    const int total = Hi * Wi;
+    const float sy = (float)H / (float)Hi, sx = (float)W / (float)Wi;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+        const int oy = i / Wi, ox = i - oy * Wi;
+        int iy = (int)floorf(oy * sy), ix = (int)floorf(ox * sx);
+        iy = iy < H - 1 ? iy : H - 1;
+        ix = ix < W - 1 ? ix : W - 1;
+        int base = 0;
+        if (lo) {
+            int y0, y1, x0, x1;
+            float ly, lx;
+            bl_src(iy, h, H, align, y0, y1, ly);
+            bl_src(ix, w, W, align, x0, x1, lx);
+            const size_t plane = (size_t)h * w;
+            float mx = -INFINITY;
+            for (int c = 0; c < NC; ++c) mx = fmaxf(mx, tta_sample(lo + c * plane, w, y0, y1, x0, x1, ly, lx));
+            float sum = 0.f;
+            for (int c = 0; c < NC; ++c) sum += expf(tta_sample(lo + c * plane, w, y0, y1, x0, x1, ly, lx) - mx);
+            float best = -INFINITY;
+            for (int c = 0; c < NC; ++c) {
+                const float p = expf(tta_sample(lo + c * plane, w, y0, y1, x0, x1, ly, lx) - mx) / sum;
+                if (p > best) { best = p; base = c; }
+            }
+        }
+        const float n = new_label ? new_label[(size_t)iy * W + (flip ? W - 1 - ix : ix)] : 0.f;
+        out[i] = n != 0.f ? n : (float)base;
+    }
+}
+
 
 // soft_logit_aggregation (aot_engine.py:565-582) for E sub-engines of max_obj objects each, fused: per output pixel
 //   prob_e = softmax over the 1 + max_obj channels of engine e;  bg = prod_e prob_e[0];
@@ -421,6 +524,34 @@ extern "C" int aotb_nearest_resize_f32(const float* in, float* out, int H, int W
     AOTB_REQUIRE(in && out && H > 0 && W > 0 && Ho > 0 && Wo > 0, "aotb_nearest_resize_f32: bad args");
     launch(nearest_kernel, dim3(cdiv(Ho * Wo, 256)), dim3(256), 0, (cudaStream_t)stream, in, out, H, W, Ho, Wo);
     return check_launch("aotb_nearest_resize_f32");
+}
+
+extern "C" int aotb_tta_merge_f32(const float* const* logits, const int* sizes, const int* flips, int n_augs, int NC, int H,
+                                  int W, int align_corners, const float* new_label, float* label, float* pred_prob,
+                                  void* stream) {
+    AOTB_REQUIRE(logits && sizes && flips && label && NC > 0 && H > 0 && W > 0, "aotb_tta_merge_f32: bad args");
+    AOTB_REQUIRE(n_augs >= 1 && n_augs <= 8, "aotb_tta_merge_f32: 1 to 8 augmentations (got %d)", n_augs);
+    TTAArgs a;
+    for (int e = 0; e < 8; ++e) {
+        const bool live = e < n_augs;
+        a.logits[e] = live ? logits[e] : nullptr;
+        a.h[e] = live ? sizes[2 * e] : 1;
+        a.w[e] = live ? sizes[2 * e + 1] : 1;
+        a.flip[e] = live ? (flips[e] != 0) : 0;
+        AOTB_REQUIRE(!live || (a.logits[e] && a.h[e] > 0 && a.w[e] > 0), "aotb_tta_merge_f32: augmentation %d: bad map", e);
+    }
+    launch(tta_merge_kernel, dim3(cdiv(H * W, 256)), dim3(256), 0, (cudaStream_t)stream, a, n_augs, NC, H, W, align_corners,
+           new_label, label, pred_prob);
+    return check_launch("aotb_tta_merge_f32");
+}
+
+extern "C" int aotb_tta_feedback_f32(const float* logits, int h, int w, int NC, int H, int W, int align_corners, int flip,
+                                     const float* new_label, float* out, int Hi, int Wi, void* stream) {
+    AOTB_REQUIRE(out && H > 0 && W > 0 && Hi > 0 && Wi > 0, "aotb_tta_feedback_f32: bad args");
+    AOTB_REQUIRE(!logits || (h > 0 && w > 0 && NC > 0), "aotb_tta_feedback_f32: bad logit map");
+    launch(tta_feedback_kernel, dim3(cdiv(Hi * Wi, 256)), dim3(256), 0, (cudaStream_t)stream, logits, h, w, NC, H, W,
+           align_corners, flip ? 1 : 0, new_label, out, Hi, Wi);
+    return check_launch("aotb_tta_feedback_f32");
 }
 
 

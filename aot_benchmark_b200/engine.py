@@ -149,6 +149,31 @@ def _cur_stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+def fork_join(owner, items, fn):
+    """fn(index, item) for every item: item 0 on the current stream, the others concurrently on side streams owned by `owner`
+    (created once, kept across calls), forked from and joined to the current stream.  fn may fork again: a nested call forks
+    from the side stream it runs on, onto its own owner's streams.  Sequential on the current stream for one item or with
+    AOTB_SUB_ENGINE_STREAMS=0."""
+    if len(items) == 1 or not SUB_ENGINE_STREAMS:
+        return [fn(i, x) for i, x in enumerate(items)]
+    cur = torch.cuda.current_stream()
+    side = getattr(owner, "_side_streams", [])
+    while len(side) < len(items) - 1:
+        side.append(torch.cuda.Stream())
+    owner._side_streams = side
+    side = side[: len(items) - 1]
+    for s in side:
+        s.wait_stream(cur)                      # fork: everything queued so far (shared encoding, masks) is visible
+    outs = [None] * len(items)
+    for i in range(1, len(items)):
+        with torch.cuda.stream(side[i - 1]):
+            outs[i] = fn(i, items[i])
+    outs[0] = fn(0, items[0])
+    for s in side:
+        cur.wait_stream(s)                      # join
+    return outs
+
+
 def lt_splits(n_queries, heads, tk, sms=132, variant=None):
     """KV-split count for the tensor-core kernel: fill whole waves of CTA slots while keeping >= 2 x 128 keys per split.
     One CTA = 128 queries x 1 head x 1 split at one CTA per SM ("tile" / "groups" / "ahead" layouts) or 64 queries x 1
@@ -1383,31 +1408,9 @@ class AOTInferEngine(nn.Module):
     # every sub-engine after the first runs on its own side stream (forked from and joined to the caller's stream inside
     # each protocol call) and the small per-engine kernels overlap on the GPU instead of queueing behind one another as in
     # the reference's Python loop (aot_engine.py:584-630); mask separation and logit aggregation are one kernel each.
-    def _engine_streams(self):
-        n = len(self.aot_engines)
-        pool = getattr(self, "_side_streams", [])
-        while len(pool) < n - 1:
-            pool.append(torch.cuda.Stream())
-        self._side_streams = pool
-        return pool[: n - 1]
-
     def _run_engines(self, fn):
         """fn(index, engine) for every sub-engine; engine 0 on the current stream, the others concurrently on side streams."""
-        engines = self.aot_engines
-        if len(engines) == 1 or not SUB_ENGINE_STREAMS:
-            return [fn(i, e) for i, e in enumerate(engines)]
-        cur = torch.cuda.current_stream()
-        side = self._engine_streams()
-        for s in side:
-            s.wait_stream(cur)                      # fork: everything queued so far (shared encoding, masks) is visible
-        outs = [None] * len(engines)
-        for i in range(1, len(engines)):
-            with torch.cuda.stream(side[i - 1]):
-                outs[i] = fn(i, engines[i])
-        outs[0] = fn(0, engines[0])
-        for s in side:
-            cur.wait_stream(s)                      # join
-        return outs
+        return fork_join(self, self.aot_engines, fn)
 
     def separate_mask(self, mask, obj_nums):
         """aot_engine.py:515-545 -> (per-engine masks, per-engine object counts).  Label maps go through one kernel

@@ -558,6 +558,53 @@ def soft_logit_aggregation(logits, out, max_obj, stream=None):
     return out
 
 
+def tta_merge(logits, flips, label, align_corners, new_label=None, prob=None, stream=None):
+    """Test-time augmentation ensemble: logits = list of E (1..8) contiguous maps [NC, h_e, w_e] (leading dims of size 1, one
+    NC for all), flips = E bools; label [H, W] = first argmax of the mean softmax of the bilinear upsamples (flipped ones read
+    mirrored), overwritten by new_label [H, W] where that is nonzero; prob [NC, H, W] receives the mean probabilities."""
+    import ctypes
+    _chk(label, new_label, prob, *logits)
+    E = len(logits)
+    if not 1 <= E <= 8 or len(flips) != E:
+        raise AotbError(f"tta_merge: 1 to 8 logit maps with one flip bit each, got {E} maps and {len(flips)} flips")
+    for t in logits:
+        _dense_maps("tta_merge logits", t, (logits[0].shape[-3], None, None))
+    NC = int(logits[0].shape[-3])
+    H, W = label.shape[-2:]
+    for name, t in (("label", label), ("new_label", new_label)):
+        if t is not None and (t.numel() != H * W or not t.is_contiguous() or tuple(t.shape[-2:]) != (H, W)):
+            raise AotbError(f"tta_merge: {name} must be one contiguous [{H}, {W}] map, got {tuple(t.shape)}")
+    if prob is not None:
+        _dense_maps("tta_merge prob", prob, (NC, H, W))
+    arr = (ctypes.c_void_p * E)(*[t.data_ptr() for t in logits])
+    sizes = (ctypes.c_int * (2 * E))(*[int(v) for t in logits for v in t.shape[-2:]])
+    fl = (ctypes.c_int * E)(*[1 if f else 0 for f in flips])
+    check(lib().aotb_tta_merge_f32(arr, sizes, fl, E, NC, H, W, 1 if align_corners else 0, _p(new_label), _p(label), _p(prob),
+                                   _st(stream)), "aotb_tta_merge_f32")
+    return label
+
+
+def tta_feedback(logits, out, output_size, align_corners, flip, new_label=None, stream=None):
+    """One augmentation's memory label: out [Hi, Wi] = nearest resize from output_size (H, W) of (new_label mirrored if flip,
+    where nonzero, else argmax softmax of the bilinear upsample of logits [NC, h, w] to (H, W)).  logits None: background (the
+    first frame's form); new_label None: no new objects."""
+    _chk(logits, out, new_label)
+    H, W = int(output_size[0]), int(output_size[1])
+    Hi, Wi = out.shape[-2:]
+    if out.numel() != Hi * Wi or not out.is_contiguous():
+        raise AotbError(f"tta_feedback: out must be one contiguous [Hi, Wi] map, got {tuple(out.shape)}")
+    if new_label is not None and (new_label.numel() != H * W or not new_label.is_contiguous()
+                                  or tuple(new_label.shape[-2:]) != (H, W)):
+        raise AotbError(f"tta_feedback: new_label must be one contiguous [{H}, {W}] map, got {tuple(new_label.shape)}")
+    NC, h, w = 0, 0, 0
+    if logits is not None:
+        _dense_maps("tta_feedback logits", logits, (None, None, None))
+        NC, h, w = (int(v) for v in logits.shape[-3:])
+    check(lib().aotb_tta_feedback_f32(_p(logits), h, w, NC, H, W, 1 if align_corners else 0, 1 if flip else 0, _p(new_label),
+                                      _p(out), Hi, Wi, _st(stream)), "aotb_tta_feedback_f32")
+    return out
+
+
 def separate_labels(mask, out, max_obj, stream=None):
     """mask: contiguous label map with HW elements; out [E, ...HW...] receives the per-engine renumbered label maps."""
     _chk(mask, out)

@@ -224,6 +224,20 @@ int aotb_preprocess_bgr_u8(const void* img, int H, int W, const int* ix, const f
 int aotb_label_to_u8(const float* label, void* out_u8, int n, void* stream);
 /* F.interpolate(mode="nearest") of a label map: networks/managers/evaluator.py:418-421. */
 int aotb_nearest_resize_f32(const float* in, float* out, int H, int W, int Ho, int Wo, void* stream);
+/* Test-time augmentation ensemble, networks/managers/evaluator.py:332-369, in one pass: n_augs (1..8) logit maps
+ * logits[e] -> [NC][h_e][w_e] fp32 on the device, with sizes[2e], sizes[2e+1] = h_e, w_e and flips[e] (the three arrays are host
+ * memory); per output pixel (y, x) of [H][W]: augmentation e is upsampled bilinearly at column flips[e] ? W-1-x : x (:333-337),
+ * softmaxed over NC (:339), the probabilities averaged in augmentation order (:355-358); label = first argmax (:359-361), then
+ * new_label[i] where that is nonzero (:363-369; new_label may be null).  pred_prob [NC][H][W] is written when not null.
+ * A map already at [H][W] (the aggregated logits of a > 10-object engine) is read unchanged. */
+int aotb_tta_merge_f32(const float* const* logits, const int* sizes, const int* flips, int n_augs, int NC, int H, int W,
+                       int align_corners, const float* new_label, float* label, float* pred_prob, void* stream);
+/* One augmentation's memory label, networks/managers/evaluator.py:346-353 and :363-422 (:315-319 on the first frame): for
+ * each pixel of out [Hi][Wi] take its nearest source (sy, sx) in [H][W] (the rule of aotb_nearest_resize_f32); base =
+ * argmax softmax of the bilinear upsample of logits [NC][h][w] at (sy, sx), or 0 when logits is null; n = new_label[sy][flip ?
+ * W-1-sx : sx], or 0 when new_label is null; out = n != 0 ? n : base. */
+int aotb_tta_feedback_f32(const float* logits, int h, int w, int NC, int H, int W, int align_corners, int flip,
+                          const float* new_label, float* out, int Hi, int Wi, void* stream);
 
 /* Tensor-core long-term attention (wgmma + TMA), AOT head shape H x 32, split-fp16 ("fp16x2")
  * operands: every fp32 value x is stored as hi = fp16(x), lo = fp16(x - hi) in rows [hi(32) | lo(32)].
