@@ -26,6 +26,11 @@
 // per CTA) of loads in flight while it splits and stores the third, which is 96 registers per thread.
 // The N tile sets how often the activations are gathered: a layer with Cout = 256 reads its input once at BN = 256 and four
 // times at BN = 64.  STAGES: 4 at BN = 64, 3 at 128, 2 at 256 (a stage is 32 KB of A plus BN * 256 bytes of B).
+//
+// Single-pass mode (SPLIT = false, selected by wl == NULL): the producer stores hi = fp16(x) only, the TMA thread streams Wh
+// only and the consumers issue Ah Wh once per k-step.  Products are then fp16 x fp16 with fp32 accumulation: each operand
+// carries 2^-11 relative rounding (the weights keep their per-channel normalisation, so any scale gets it).  A stage is
+// 16 KB of A plus BN * 128 bytes of B, so the same budget holds twice the chunks: STAGES 8 at BN = 64, 6 at 128, 4 at 256.
 #include <type_traits>
 
 #include "common.cuh"
@@ -187,21 +192,22 @@ __device__ __forceinline__ void conv_finish_tile_pre(const ConvTcArgs& a, const 
     }
 }
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool SPLIT>
 struct ConvSmem {
     static constexpr int A_BYTES = CONV_A_BYTES;
     static constexpr int B_BYTES = BN * 128;
-    static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
+    static constexpr int PARTS = SPLIT ? 2 : 1;        // hi and lo tiles, or hi only
+    static constexpr int STAGE_BYTES = PARTS * A_BYTES + PARTS * B_BYTES;
     static constexpr int STG_LD = BN + 4;              // staging tile [128][BN + 4] fp32, aliases the stages
     static_assert(128 * STG_LD * 4 <= STAGES * STAGE_BYTES, "staging tile must fit in the operand stages");
     static constexpr int TOTAL = STAGES * STAGE_BYTES + 128 * (int)sizeof(RowInfo) + 3 * STAGES * 8 + 1024;
     static_assert(TOTAL <= 227 * 1024, "shared memory of one CTA");
 };
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool SPLIT>
 __global__ void __launch_bounds__(384, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const ConvTcArgs a) {
-    using SM = ConvSmem<BN, STAGES>;
+    using SM = ConvSmem<BN, STAGES, SPLIT>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     RowInfo* rinfo = reinterpret_cast<RowInfo*>(smem + STAGES * SM::STAGE_BYTES);
@@ -250,7 +256,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
     if (wg < 2) {
         // ======================= consumers: wgmma only =======================
         const uint64_t dA0 = smem_desc_sw128(smem_u32(smem + wg * 64 * 128));
-        const uint64_t dB0 = smem_desc_sw128(smem_u32(smem + 2 * SM::A_BYTES));
+        const uint64_t dB0 = smem_desc_sw128(smem_u32(smem + SM::PARTS * SM::A_BYTES));
         float acc[BN / 2];
 #pragma unroll
         for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
@@ -268,8 +274,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
 #pragma unroll
             for (int ks = 0; ks < 4; ++ks) {
                 wgmma_conv<BN>(acc, ah + 2 * ks, bh + 2 * ks);
-                wgmma_conv<BN>(acc, al + 2 * ks, bh + 2 * ks);
-                wgmma_conv<BN>(acc, ah + 2 * ks, bl + 2 * ks);
+                if constexpr (SPLIT) {
+                    wgmma_conv<BN>(acc, al + 2 * ks, bh + 2 * ks);
+                    wgmma_conv<BN>(acc, ah + 2 * ks, bl + 2 * ks);
+                }
             }
             wgmma_commit();
             reg_fence<BN / 2>(acc);
@@ -297,7 +305,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
         // recomputed only when the tap changes (never for 1x1 convs and linears, every Cin/64 chunks for 3x3)
         uint32_t off[16];
         int cur_tap = -1, c4 = 0;
-        if (p == 0) { tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl); }
+        if (p == 0) { tma_prefetch_desc(&tmWh); if constexpr (SPLIT) tma_prefetch_desc(&tmWl); }
         auto load_half = [&](int h, auto part_c, float4* v) {
             constexpr int part = decltype(part_c)::value;
             if (part == 0) {
@@ -333,10 +341,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
             if (part == 0) {
                 if (it >= STAGES) mbar_wait_cp(&s_free[s], ((it / STAGES) - 1) & 1, a.spin);
                 if (p == 0) {
-                    uint8_t* Bh = stage + 2 * SM::A_BYTES;
-                    mbar_arrive_expect_tx(&b_full[s], 2 * SM::B_BYTES);
+                    uint8_t* Bh = stage + SM::PARTS * SM::A_BYTES;
+                    mbar_arrive_expect_tx(&b_full[s], SM::PARTS * SM::B_BYTES);
                     tma_load_2d(Bh, &tmWh, &b_full[s], (kbeg + it) * 64, n0);
-                    tma_load_2d(Bh + SM::B_BYTES, &tmWl, &b_full[s], (kbeg + it) * 64, n0);
+                    if constexpr (SPLIT) tma_load_2d(Bh + SM::B_BYTES, &tmWl, &b_full[s], (kbeg + it) * 64, n0);
                 }
             }
             uint8_t* Ah = stage + part * 64 * 128 + soff;
@@ -344,6 +352,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 const __half2 h0 = __floats2half2_rn(v[i].x, v[i].y), h1 = __floats2half2_rn(v[i].z, v[i].w);
+                if constexpr (!SPLIT) {
+                    uint2 ph;
+                    ph.x = *reinterpret_cast<const uint32_t*>(&h0); ph.y = *reinterpret_cast<const uint32_t*>(&h1);
+                    *reinterpret_cast<uint2*>(Ah + i * 1024) = ph;
+                    continue;
+                }
                 const __half2 l0 = __floats2half2_rn(v[i].x - __low2float(h0), v[i].y - __high2float(h0));
                 const __half2 l1 = __floats2half2_rn(v[i].z - __low2float(h1), v[i].w - __high2float(h1));
                 uint2 ph, pl;
@@ -423,12 +437,13 @@ static int make_tmap_weights(CUtensorMap* out, const void* base, int Kpad, int C
     return AOTB_OK;
 }
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool SPLIT>
 static int launch_conv_tc(const CUtensorMap& th, const CUtensorMap& tl, const ConvTcArgs& a, cudaStream_t st) {
-    constexpr int smem = ConvSmem<BN, STAGES>::TOTAL;
+    constexpr int smem = ConvSmem<BN, STAGES, SPLIT>::TOTAL;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             smem);
         if (e != cudaSuccess) {
             set_error("aotb_conv2d_nhwc_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
             return AOTB_ERR_CUDA;
@@ -436,7 +451,7 @@ static int launch_conv_tc(const CUtensorMap& th, const CUtensorMap& tl, const Co
         configured = true;
     }
     dim3 grid(cdiv(a.M, 128), a.Cout / BN, a.splits);
-    launch_cluster(conv_tc_kernel<BN, STAGES>, dim3(grid), dim3(384), smem, st, a.splits, th, tl, a);
+    launch_cluster(conv_tc_kernel<BN, STAGES, SPLIT>, dim3(grid), dim3(384), smem, st, a.splits, th, tl, a);
     return check_launch("aotb_conv2d_nhwc_tc");
 }
 
@@ -452,12 +467,13 @@ extern "C" int aotb_set_conv_tiling(int mode) {
 }
 
 // wh / wl: pre-split weights [Cout][Kpad] fp16 (K = KH*KW*Cin ordered (ky,kx,ci), zero-padded to a multiple of 64);
-// wscale [Cout]: per-channel factor of the accumulator (null = 1).
+// wl == null selects the single-pass kernel (hi operands only); wscale [Cout]: per-channel factor of the accumulator (null = 1).
 extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* wl, const float* bias, const float* wscale,
                                    const float* res, float* out, int B, int H, int W, int Cin, int ldin, int Cout, int ldout, int ldres,
                                    int KH, int KW, int stride, int pad, int act, void* workspace, size_t workspace_bytes,
                                    void* stream) {
-    AOTB_REQUIRE(in && wh && wl && out, "aotb_conv2d_nhwc_tc: null pointer");
+    AOTB_REQUIRE(in && wh && out, "aotb_conv2d_nhwc_tc: null pointer");
+    const bool split = wl != nullptr;
     AOTB_REQUIRE(Cin % 4 == 0 && Cout % 64 == 0, "aotb_conv2d_nhwc_tc: Cin must be a multiple of 4, Cout of 64");
     AOTB_REQUIRE(act >= aotb::ACT_NONE && act <= aotb::ACT_RELU6, "aotb_conv2d_nhwc_tc: activation %d not supported (0-4)", act);
     AOTB_REQUIRE(ldin % 4 == 0 && ldout % 4 == 0 && (!res || ldres % 4 == 0) && ((uintptr_t)in % 16 == 0) &&
@@ -485,13 +501,18 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     // with scripts/conv_sweep.py on an H100 (80GB HBM3, 700 W): over the 20 conv / linear shapes of an R50-AOTL 480p frame
     // the policy's tiles take 632 us in total against 632 us for the best measured tiling of each shape.  Bit 0 of the
     // tuning mask ("narrow") selects the simpler heuristic instead.
+    // The single-pass kernel has its own row: one MMA per k-step (a third of the units) and its own gather constant
+    // kGather1 (half the shared-memory stores, no lo split), so every tile is gather-bound and the choice turns on waves
+    // and finish cost.  Checked with scripts/conv_sweep.py --single-pass on the same card and shapes: the policy's tiles
+    // take 478 us against 473 us for the best measured tiling of each shape (the split kernel's policy: 633 us).
     const int mt = cdiv(a.M, 128);
     int BN = 64, best_s = 1;
-    const float kGather = 2.5f;
+    const float kGather = 2.5f, kGather1 = 2.0f;
     if ((tc::g_conv_tiling & 1) == 0) {
         float best = 1e30f;
         const int bns[3] = {256, 128, 64};
         const float t_chunk[3] = {fmaxf(kGather, 4.0f), fmaxf(kGather, 2.0f), fmaxf(kGather, 1.0f)};
+        const float t_chunk1[3] = {fmaxf(kGather1, 4.0f / 3), fmaxf(kGather1, 2.0f / 3), fmaxf(kGather1, 1.0f / 3)};
         const float t_fin[3] = {8.0f, 4.0f, 2.0f};
         for (int bi = 0; bi < 3; ++bi) {
             if (Cout % bns[bi]) continue;
@@ -501,7 +522,7 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
                 const int slots = sp == 8 ? 128 : 132;                        // co-resident CTAs with clusters of sp
                 if (sp > 1 && ctas > slots) continue;                         // split-K only to fill a partial wave
                 const int waves = cdiv(ctas, slots);
-                const float t = waves * (3.0f + cdiv(a.nchunks, sp) * t_chunk[bi] + t_fin[bi]);
+                const float t = waves * (3.0f + cdiv(a.nchunks, sp) * (split ? t_chunk[bi] : t_chunk1[bi]) + t_fin[bi]);
                 if (t < best) { best = t; BN = bns[bi]; best_s = sp; }
             }
         }
@@ -535,9 +556,14 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     CUtensorMap th, tl;
     int rc;
     if ((rc = tc::make_tmap_weights(&th, wh, K, Cout, BN)) != AOTB_OK) return rc;
-    if ((rc = tc::make_tmap_weights(&tl, wl, K, Cout, BN)) != AOTB_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    if (BN == 256) return tc::launch_conv_tc<256, 2>(th, tl, a, st);
-    if (BN == 128) return tc::launch_conv_tc<128, 3>(th, tl, a, st);
-    return tc::launch_conv_tc<64, 4>(th, tl, a, st);
+    if (!split) {             // the kernel never reads tmWl
+        if (BN == 256) return tc::launch_conv_tc<256, 4, false>(th, th, a, st);
+        if (BN == 128) return tc::launch_conv_tc<128, 6, false>(th, th, a, st);
+        return tc::launch_conv_tc<64, 8, false>(th, th, a, st);
+    }
+    if ((rc = tc::make_tmap_weights(&tl, wl, K, Cout, BN)) != AOTB_OK) return rc;
+    if (BN == 256) return tc::launch_conv_tc<256, 2, true>(th, tl, a, st);
+    if (BN == 128) return tc::launch_conv_tc<128, 3, true>(th, tl, a, st);
+    return tc::launch_conv_tc<64, 4, true>(th, tl, a, st);
 }

@@ -16,6 +16,7 @@ Training (AOTEngine.forward, aot_engine.py:33-108) is a "next" row of SURVEY 8(f
 """
 from __future__ import annotations
 
+import functools
 import math
 
 import numpy as np
@@ -105,6 +106,39 @@ def _resolve_mem_max(aot_model, long_term_mem_max):
     if int(m) != m or m < 2:
         raise ValueError(f"long_term_mem_max must be an integer >= 2 (the first memory frame and at least one recent one), got {m}")
     return int(m)
+
+
+def _resolve_precision(aot_model, precision):
+    """The engine's precision: the keyword, else cfg.TEST_PRECISION, else "fp32".  "fp16" runs every tensor-core conv and
+    linear with operands rounded once to fp16 and the tensor-core attention without its exact (lo) terms; it does not
+    follow torch.is_autocast_enabled()."""
+    p = getattr(aot_model.cfg, "TEST_PRECISION", None) if precision is None else precision
+    if p is None:
+        return "fp32"
+    if p not in ops.PRECISIONS:
+        raise ValueError(f"precision must be one of {ops.PRECISIONS}, got {p!r}")
+    if p == "fp16":
+        # the fp16 mode is built from the tensor-core kernels only; these knobs select fp32 CUDA-core or split-GEMM paths
+        if ops.CONV_IMPL == "simt":
+            raise NotImplementedError("precision='fp16' runs the tensor-core conv; AOTB_CONV_IMPL=simt selects the fp32 "
+                                      "CUDA-core conv")
+        if LT_IMPL == "simt":
+            raise NotImplementedError("precision='fp16' runs the tensor-core long-term attention; AOTB_LT_IMPL=simt selects "
+                                      "the fp32 CUDA-core kernel")
+        if aot_model.cfg.MODEL_VOS == "deaot" and DEAOT_LT in ("gemm", "simt"):
+            raise NotImplementedError(f"precision='fp16' runs DeAOT's attention on the fused tensor-core kernel; "
+                                      f"AOTB_DEAOT_LT={DEAOT_LT} selects another path")
+    return p
+
+
+def _in_precision(fn):
+    """Run an engine method with the tensor-core conv / linear launches it issues (graph captures included) in the
+    engine's precision."""
+    @functools.wraps(fn)
+    def wrapper(self, *args, **kwargs):
+        with ops.precision(self.precision):
+            return fn(self, *args, **kwargs)
+    return wrapper
 
 
 REPLAYED_KERNELS = [0]      # kernels launched through graph replays (bench.py adds this to the library's eager count)
@@ -468,11 +502,16 @@ class _Encoder:
 # single engine (<= max_obj_num objects)
 # =====================================================================================
 class AOTEngine(nn.Module):
-    def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1, long_term_mem_max=None):
+    def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1, long_term_mem_max=None,
+                 precision=None):
         """long_term_mem_max = M bounds the long-term bank to M memory frames: the first frame stored after
         restart_engine() stays, the other M - 1 slots hold the newest stored frames (the oldest is overwritten).  None: the
-        bound of cfg.TEST_LONG_TERM_MEM_MAX if the config has one, else the reference's ever-growing memory."""
+        bound of cfg.TEST_LONG_TERM_MEM_MAX if the config has one, else the reference's ever-growing memory.
+        precision: "fp32" (default; split-fp16 tensor-core operands, fp32-faithful) or "fp16" (operands of every
+        tensor-core conv, linear and attention product rounded once to fp16, accumulated in fp32).  None: cfg.TEST_PRECISION
+        if the config has one, else "fp32"."""
         super().__init__()
+        self.precision = _resolve_precision(aot_model, precision)
         self.cfg = aot_model.cfg
         self.align_corners = aot_model.cfg.MODEL_ALIGN_CORNERS
         self.AOT = aot_model
@@ -526,6 +565,8 @@ class AOTEngine(nn.Module):
         runs the rest of the network redundantly on identical inputs; rank `f % world` keeps memory frame f; each
         rank's long-term attention produces un-normalised partials (m, l, O) over its shard which are all-gathered
         (one NCCL collective per layer) and merged exactly (log-sum-exp) on every rank."""
+        if self.precision == "fp16":
+            raise NotImplementedError("a long-term bank sharded over GPUs is not built for precision='fp16'")
         if not (LT_IMPL.startswith("tc") and not self._plan_is_deaot()):
             raise NotImplementedError("sharded long-term attention is implemented for the AOT tensor-core kernel")
         if self.long_term_mem_max is not None:
@@ -735,6 +776,7 @@ class AOTEngine(nn.Module):
         return out
 
     # ------------------------------------------------------------------ steps
+    @_in_precision
     def _encode(self, img, st):
         if self._enc is None:
             self._enc = _Encoder(self._plan(), img.shape[2], img.shape[3])
@@ -745,6 +787,7 @@ class AOTEngine(nn.Module):
         if not img.is_cuda:
             raise RuntimeError("aot_benchmark_b200 engines run on CUDA tensors only (there is no CPU path)")
 
+    @_in_precision
     def assign_identity_from_mask(self, mask, st):
         """one_hot_mask + get_id_emb (aot_engine.py:168-179) fused as a gather (K4)."""
         P = self._plan()
@@ -775,6 +818,7 @@ class AOTEngine(nn.Module):
             ops.id_embed(m2, P.id_wt, P.id_b, self._ws.id_emb, P.C, P.nid, P.id_k, P.id_stride, P.id_pad,
                          ln_gamma=P.id_norm[0] if P.deaot else None, ln_beta=P.id_norm[1] if P.deaot else None, stream=st)
 
+    @_in_precision
     def add_reference_frame(self, img=None, mask=None, frame_step=-1, obj_nums=None, img_embs=None):
         if self.obj_nums is None and obj_nums is None:
             print('No objects for reference frame!')
@@ -818,6 +862,7 @@ class AOTEngine(nn.Module):
         self.last_mem_step = self.frame_step
         self._have_lstt = True
 
+    @_in_precision
     def match_propogate_one_frame(self, img=None, img_embs=None):
         self.frame_step += 1
         st = torch.cuda.current_stream().cuda_stream
@@ -836,6 +881,7 @@ class AOTEngine(nn.Module):
                         lambda: self._lstt_forward(img_embs, None, _cur_stream()),
                         enabled=self.short_term_mem_skip <= 1 and (self.kv_shard is None or SHARD_GRAPHS))
 
+    @_in_precision
     def update_short_term_memory(self, curr_mask, curr_id_emb=None, skip_long_term_update=False):
         st = torch.cuda.current_stream().cuda_stream
         append = False
@@ -1017,8 +1063,8 @@ class AOTEngine(nn.Module):
                 fz = lambda *s: torch.empty(s, dtype=torch.float32, device=out.device)
                 part = (fz(splits, N, P.C), fz(splits, P.H, N), fz(splits, P.H, N))
                 ws.part[splits] = part
-        ops.lt_attention_tc(ws.Qp, Kp, Vp, N, Tk, O=out, Tk_dev=Tk_dev, splits=splits, exact=(LT_IMPL == "tc_exact"),
-                            part=part, stream=st)
+        exact = LT_IMPL == "tc_exact" and self.precision == "fp32"
+        ops.lt_attention_tc(ws.Qp, Kp, Vp, N, Tk, O=out, Tk_dev=Tk_dev, splits=splits, exact=exact, part=part, stream=st)
 
     def _shard_splits(self):
         """KV-split count of the per-rank partial attention in sharded mode: a function of the GLOBAL memory-frame count, so it
@@ -1172,6 +1218,7 @@ class AOTEngine(nn.Module):
         ops.conv2d(x, D.conv_out.w, D.conv_out.b, lg, stream=st)
         return lg
 
+    @_in_precision
     def decode_current_logits(self, output_size=None):
         """aot_engine.py:356-380.  The returned tensor (and ``pred_id_logits``) are per-engine static buffers that
         the next call overwrites -- clone them to keep a frame's logits."""
@@ -1215,8 +1262,9 @@ class DeAOTEngine(AOTEngine):
     """networks/engines/deaot_engine.py:9-56 -- GatedPropagationModule stack (transformer.py:501-665)."""
 
     def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1,
-                 layer_loss_scaling_ratio=2., long_term_mem_max=None):
-        super().__init__(aot_model, gpu_id, long_term_mem_gap, short_term_mem_skip, long_term_mem_max=long_term_mem_max)
+                 layer_loss_scaling_ratio=2., long_term_mem_max=None, precision=None):
+        super().__init__(aot_model, gpu_id, long_term_mem_gap, short_term_mem_skip, long_term_mem_max=long_term_mem_max,
+                         precision=precision)
         self.layer_loss_scaling_ratio = layer_loss_scaling_ratio
 
     def _gated_tail(self, core, U, dw_w, out_slice, h, w, st):
@@ -1331,7 +1379,8 @@ class DeAOTEngine(AOTEngine):
             if part is None:
                 fz = lambda *s: torch.empty(s, dtype=torch.float32, device=out.device)
                 part = ws.gp_part[splits] = (fz(splits, N, out.shape[1]), fz(splits, 1, N), fz(splits, 1, N))
-        ops.gp_attention_tc(ws.gpQp, Kp, Vp, N, Tk, O=out, Tk_dev=Tk_dev, splits=splits, exact=True, part=part, stream=st)
+        ops.gp_attention_tc(ws.gpQp, Kp, Vp, N, Tk, O=out, Tk_dev=Tk_dev, splits=splits, exact=self.precision == "fp32",
+                            part=part, stream=st)
 
     def _gp_splits(self, Tk):
         """KV-split count of the fused DeAOT long-term attention kernel (one CTA = 128 queries x 64 value channels x one
@@ -1371,9 +1420,11 @@ class AOTInferEngine(nn.Module):
     _engine_cls = AOTEngine
 
     def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1, max_aot_obj_num=None,
-                 long_term_mem_max=None):
-        """long_term_mem_max: bound of every sub-engine's long-term bank in memory frames (see AOTEngine)."""
+                 long_term_mem_max=None, precision=None):
+        """long_term_mem_max: bound of every sub-engine's long-term bank in memory frames; precision: "fp32" | "fp16" of
+        every sub-engine (see AOTEngine for both)."""
         super().__init__()
+        self.precision = _resolve_precision(aot_model, precision)
         self.cfg = aot_model.cfg
         self.AOT = aot_model
         if max_aot_obj_num is None or max_aot_obj_num > aot_model.max_obj_num:
@@ -1390,6 +1441,8 @@ class AOTInferEngine(nn.Module):
 
     def enable_kv_sharding(self, rank, world, group=None):
         """Shard the long-term memory bank over `world` ranks (see AOTEngine.enable_kv_sharding)."""
+        if self.precision == "fp16":
+            raise NotImplementedError("a long-term bank sharded over GPUs is not built for precision='fp16'")
         if self.long_term_mem_max is not None:
             raise NotImplementedError("a bounded long-term bank (long_term_mem_max) cannot be sharded over GPUs: each rank "
                                       "would need its own ring")
@@ -1456,7 +1509,8 @@ class AOTInferEngine(nn.Module):
         while len(self.aot_engines) < want:
             eng = self._pool.pop(0) if self._pool else self._engine_cls(self.AOT, self.gpu_id, self.long_term_mem_gap,
                                                                        self.short_term_mem_skip,
-                                                                       long_term_mem_max=self.long_term_mem_max)
+                                                                       long_term_mem_max=self.long_term_mem_max,
+                                                                       precision=self.precision)
             eng.long_term_mem_max = self.long_term_mem_max      # pooled engines too: part of their workspace key
             eng.restart_engine()
             eng.eval()

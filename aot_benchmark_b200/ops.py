@@ -10,6 +10,7 @@ operands must be contiguous (the label-map, logit post-processing and ID-embeddi
 """
 from __future__ import annotations
 
+import contextlib
 import os
 
 import torch
@@ -50,6 +51,24 @@ def _nhwc_ld(x):
 # per-channel scale (None = 1), registered by plan.py
 _TC_WEIGHTS = {}
 CONV_IMPL = os.environ.get("AOTB_CONV_IMPL", "tc")     # "tc" (wgmma, fp16x2 split) | "simt" (fp32 CUDA cores)
+PRECISIONS = ("fp32", "fp16")
+# operand precision of the tensor-core conv / linear launches issued by conv2d and linear: "fp32" = split fp16 (three MMAs,
+# fp32-faithful), "fp16" = operands rounded once (the single-pass kernel).  An engine sets it around its own calls with
+# `precision`, so two engines of different precision in one process each launch in their own mode.
+_PRECISION = "fp32"
+
+
+@contextlib.contextmanager
+def precision(p):
+    """Issue the tensor-core conv / linear launches of the enclosed calls in precision `p` ("fp32" | "fp16")."""
+    global _PRECISION
+    if p not in PRECISIONS:
+        raise ValueError(f"precision must be one of {PRECISIONS}, got {p!r}")
+    old, _PRECISION = _PRECISION, p
+    try:
+        yield
+    finally:
+        _PRECISION = old
 
 
 _TC_WS = {}
@@ -127,13 +146,14 @@ CONV_CHAIN = False
 
 
 def conv2d_tc(x, wh, wl, bias, out, res=None, KH=1, KW=1, stride=1, pad=0, act=ACT_NONE, stream=None, wscale=None):
-    """Tensor-core conv: x [B,H,W,Cin] fp32, wh/wl [Cout, KH*KW*Cin] fp16, wscale fp32 [Cout] or None (= 1)."""
+    """Tensor-core conv: x [B,H,W,Cin] fp32, wh/wl [Cout, KH*KW*Cin] fp16, wscale fp32 [Cout] or None (= 1).
+    wl None: the single-pass kernel (x rounded once to fp16, wh only)."""
     _chk(x, bias, out, res, wscale)
     B, H, W, Cin = x.shape
     Cout = wh.shape[0]
     ws = _tc_workspace(x.device)
     with _ConvProbe(2.0 * out.shape[0] * out.shape[1] * out.shape[2] * Cout * KH * KW * Cin, stream):
-        check(lib().aotb_conv2d_nhwc_tc(_p(x), wh.data_ptr(), wl.data_ptr(), _p(bias), _p(wscale), _p(res), _p(out), B, H, W, Cin,
+        check(lib().aotb_conv2d_nhwc_tc(_p(x), wh.data_ptr(), _p(wl), _p(bias), _p(wscale), _p(res), _p(out), B, H, W, Cin,
                                         _nhwc_ld(x), Cout, _nhwc_ld(out), _nhwc_ld(res) if res is not None else 0, KH, KW,
                                         stride, pad, act, ws.data_ptr(), ws.numel(), _st(stream)), "aotb_conv2d_nhwc_tc")
     return out
@@ -144,7 +164,7 @@ def conv2d(x, w, bias, out, res=None, KH=1, KW=1, stride=1, pad=0, dil=1, act=AC
     if CONV_IMPL == "tc" and dil == 1:
         t = _TC_WEIGHTS.get(w.data_ptr())
         if t is not None:
-            return conv2d_tc(x, t[0], t[1], bias, out, res=res, KH=KH, KW=KW, stride=stride, pad=pad, act=act,
+            return conv2d_tc(x, t[0], None if _PRECISION == "fp16" else t[1], bias, out, res=res, KH=KH, KW=KW, stride=stride, pad=pad, act=act,
                              stream=stream, wscale=t[2])
     _chk(x, w, bias, out, res)
     B, H, W, Cin = x.shape
@@ -165,7 +185,8 @@ def linear(x, wt, bias, out, res=None, act=ACT_NONE, stream=None):
             N = wt.shape[1]
             ws = _tc_workspace(x.device)
             with _ConvProbe(2.0 * M * N * K, stream):
-                check(lib().aotb_conv2d_nhwc_tc(_p(x), t[0].data_ptr(), t[1].data_ptr(), _p(bias), _p(t[2]), _p(res), _p(out),
+                wl = None if _PRECISION == "fp16" else t[1]
+                check(lib().aotb_conv2d_nhwc_tc(_p(x), t[0].data_ptr(), _p(wl), _p(bias), _p(t[2]), _p(res), _p(out),
                                                 1, M, 1, K, x.stride(0), N, out.stride(0), res.stride(0) if res is not None else 0,
                                                 1, 1, 1, 0, act, ws.data_ptr(), ws.numel(), _st(stream)),
                       "aotb_conv2d_nhwc_tc")

@@ -57,6 +57,10 @@ int aotb_conv2d_nhwc_f32(const float* in, const float* w, const float* bias, con
  * to 2^-25 on top of a relative 2^-22.  The normalisation takes that floor off the weights, whose products then stay
  * within ~1e-6 of fp32 for channels of any magnitude.  Activations are split as they come: elements with |x| below about
  * 2^-3 lose relative precision, and |x| >= 65520 overflows hi (inf).
+ * wl == NULL selects the single-pass kernel: activations are rounded once to hi = fp16(x), only wh is read, and each
+ * k-step issues one MMA (Ah Wh) instead of three.  Every product then carries fp16 rounding of both operands (2^-11
+ * relative; the weight normalisation still gives any channel scale that precision), accumulated in fp32.  The finish and
+ * the range are those of the split kernel; the tile policy has its own cost-model row for it.
  * Requires Cin % 4 == 0 and Cout % 64 == 0.  Few-tile deep-K layers run split-K: the 2 / 4 / 8 CTAs of one output
  * tile form a thread-block cluster and sum their partial tiles over distributed shared memory in rank order
  * (deterministic).  `workspace` / `workspace_bytes` are only used by the diagnostic mode of aotb_set_conv_tiling

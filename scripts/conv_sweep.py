@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Sweep the N tile x split-K factor of the tensor-core conv on the shapes of one R50-AOTL 480p frame (graph-replayed,
 L2-warm, CUDA events) -- the data behind the tile policy in aotb_conv2d_nhwc_tc.  GPU only; writes the rows as JSON to the
-path given as the first argument (default conv_sweep.json)."""
+path given as the first argument (default conv_sweep.json).  --single-pass also sweeps the single-pass kernel (wl = NULL, the
+fp16 inference mode) on the same shapes and inputs: one row per shape and mode."""
 import json
 import os
 import sys
@@ -44,6 +45,7 @@ def main():
     d = torch.device("cuda:0")
     g = torch.Generator().manual_seed(0)
     results = []
+    modes = ("fp32", "fp16") if "--single-pass" in sys.argv else ("fp32",)
     for name, H, W, Cin, Cout, K, s, p in SHAPES + EXTRA:
         x = torch.randn(1, H, W, Cin, generator=g).to(d)
         w = (torch.randn(K * K * Cin, Cout, generator=g) / (K * K * Cin) ** 0.5).to(d)
@@ -53,25 +55,31 @@ def main():
         out = torch.empty(1, Ho, Wo, Cout, device=d)
         nchunks = (K * K * Cin + 63) // 64
         mt = (Ho * Wo + 127) // 128
-        row = {"shape": name, "M": Ho * Wo, "K": K * K * Cin, "N": Cout, "us": {}}
-        fn = lambda: ops.conv2d_tc(x, wh, wl, b, out, KH=K, KW=K, stride=s, pad=p, act=1)  # noqa: E731
-        lib().aotb_set_conv_tiling(0)
-        row["us"]["policy"] = round(time_graph(fn), 2)
-        for bi, BN in ((1, 64), (2, 128), (3, 256)):
-            if Cout % BN:
+        for mode in modes:
+            results.append(sweep_shape(name, x, wh, wl if mode == "fp32" else None, b, out, K, s, p, Cout, nchunks, mt, mode))
+    args = [a for a in sys.argv[1:] if not a.startswith("--")]
+    json.dump(results, open(args[0] if args else "conv_sweep.json", "w"), indent=1)
+
+
+def sweep_shape(name, x, wh, wl, b, out, K, s, p, Cout, nchunks, mt, mode):
+    row = {"shape": name, "mode": mode, "M": out.shape[1] * out.shape[2], "K": K * K * x.shape[3], "N": Cout, "us": {}}
+    fn = lambda: ops.conv2d_tc(x, wh, wl, b, out, KH=K, KW=K, stride=s, pad=p, act=1)  # noqa: E731
+    lib().aotb_set_conv_tiling(0)
+    row["us"]["policy"] = round(time_graph(fn), 2)
+    for bi, BN in ((1, 64), (2, 128), (3, 256)):
+        if Cout % BN:
+            continue
+        for S in (1, 2, 4, 8):
+            ctas = mt * (Cout // BN) * S
+            if S > nchunks or (S > 1 and ctas > 320):
                 continue
-            for S in (1, 2, 4, 8):
-                ctas = mt * (Cout // BN) * S
-                if S > nchunks or (S > 1 and ctas > 320):
-                    continue
-                lib().aotb_set_conv_tiling((bi << 4) | (S << 8))
-                row["us"][f"bn{BN}_s{S}"] = round(time_graph(fn), 2)
-        lib().aotb_set_conv_tiling(0)
-        best = min(row["us"], key=row["us"].get)
-        row["best"] = best
-        results.append(row)
-        print(json.dumps(row), flush=True)
-    json.dump(results, open(sys.argv[1] if len(sys.argv) > 1 else "conv_sweep.json", "w"), indent=1)
+            lib().aotb_set_conv_tiling((bi << 4) | (S << 8))
+            row["us"][f"bn{BN}_s{S}"] = round(time_graph(fn), 2)
+    lib().aotb_set_conv_tiling(0)
+    best = min(row["us"], key=row["us"].get)
+    row["best"] = best
+    print(json.dumps(row), flush=True)
+    return row
 
 
 if __name__ == "__main__":
