@@ -12,11 +12,14 @@
 // Cin % 4 == 0, Cout % 64 == 0, dilation 1 (everything on the R50-AOTL path except the 11-channel conv_out;
 // the 7x7 stem runs on a 4-channel zero-padded copy of the image).
 //
-// One CTA = 128 output pixels x BN (64 | 128 | 256) output channels, 384 threads in three warpgroups, warp-specialised:
+// One tile = 128 output pixels x BN (64 | 128 | 256) output channels; 384 threads in three warpgroups, warp-specialised.
+// Without split-K the launch is persistent: min(tiles, SMs) CTAs, CTA b computing tiles b, b + grid, ... in a static order,
+// with one stage ring whose chunk counter and phases run on across tiles.
 //   warps 0-7   two consumer warpgroups (64 pixel rows each).  Per K chunk they wait for the stage's "A full" and "B full"
 //               barriers, issue 4 k-steps x (Ah Wh + Al Wh + Ah Wl) as wgmma m64nBNk16 and release the stage of the
-//               previous chunk on "empty" once its MMAs have completed.  Afterwards the accumulators go through a fp32
-//               staging tile in shared memory and the same warps run the finish (bias / residual / activation -> fp32 NHWC).
+//               previous chunk on "empty" once its MMAs have completed (and the tile's last stage after its final wait).
+//               Then the same warps run the finish (bias / residual / activation -> fp32 NHWC) from the accumulator
+//               registers while the producer already gathers the next tile; split-K goes through a staging tile instead.
 //   warps 8-11  producer warpgroup.  It gathers the fp32 activations of all 128 rows of a chunk straight from NHWC global
 //               memory (im2col is never materialised), splits them into hi = fp16(x), lo = fp16(x - hi), stores both
 //               128 x 64 half tiles 128B-swizzled and K-major, and arrives on "A full" after fence.proxy.async.  Thread 256
@@ -67,15 +70,18 @@ struct ConvTcArgs {
     int B, H, W, Cin, ldin;
     int Ho, Wo, Cout, ldout, ldres;
     int KH, KW, stride, pad;
-    int M, nchunks;
+    int M, mtiles, nchunks;
     int act;
     int splits;          // split-K: the `splits` CTAs (blockIdx.z) of one output tile form a thread-block cluster; CTA z
                          // handles chunks [z*per, (z+1)*per) and the partial tiles are summed over distributed smem
     int spin;            // 1: mbarrier waits without the suspend hint
+    int const_w;         // 1: no earlier kernel of the stream writes the weights (their first TMA loads precede pdl_wait)
     long long* prof;     // diagnostic: 12 clock64 stamps per CTA (see aotb_set_conv_tiling), or null
 };
 
+constexpr int AOTB_CONV_CONST_WEIGHTS = 256;       // flag in the act argument (include/aotb200.h)
 static int g_conv_tiling = 0;      // aotb_set_conv_tiling
+static int g_conv_grid_cap = 0;    // aotb_set_conv_grid_cap (0: one CTA per SM)
 
 struct RowInfo { int pix_base, iy0, ix0, valid; };
 
@@ -127,107 +133,141 @@ __device__ __forceinline__ void conv_finish_tile(const ConvTcArgs& a, const uint
     }
 }
 
-// Finish without split-K with the global loads taken off its critical path: the bias and the residual rows of the FIRST batch are
-// already in registers (`pre`, loaded by finish_prefetch before the thread waited for the accumulator, i.e. under the tail of the
-// K loop), and inside the loop the residual rows of batch k+1 are requested before batch k is computed and stored.  The staging
-// tile is read with ld.shared so that the compiler does not have to order those reads behind the global stores.
-// Rows per batch: 4 at BN = 256, where the prefetched rows sit beside 128 accumulator registers.
-template <int BN>
-struct FinishPre { static constexpr int B = BN == 256 ? 4 : 8; float4 b4, s4; float4 rs[B]; };
+__device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 
-template <int BN>
-__device__ __forceinline__ void finish_prefetch(const ConvTcArgs& a, int tid, int m0, int n0, FinishPre<BN>& pre) {
-    constexpr int C4 = BN / 4, RSTEP = 256 / C4;
-    const int n = n0 + (tid % C4) * 4, r0 = tid / C4;
-    pre.b4 = a.bias ? __ldg(reinterpret_cast<const float4*>(a.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    pre.s4 = a.wscale ? __ldg(reinterpret_cast<const float4*>(a.wscale + n)) : make_float4(1.f, 1.f, 1.f, 1.f);
+// Finish without split-K, straight from the accumulator fragments (persistent launches: no staging tile, so the operand
+// stages stay free for the next tile's loads).  Thread (warp w, lane l) holds rows r and r + 8 (r = 64 (w / 4) + 16 (w % 4)
+// + l / 4) at columns 8 k + 2 (l % 4) + {0, 1}: one float2 per row and column group, so the four lanes of a row write a full
+// 32-byte sector.  The residual is read in the same layout, by the thread that then writes the element (an in-place
+// residual, res == out, is read before it is overwritten).  Same arithmetic per element as conv_finish_tile: bitwise equal.
+// bs: the tile's bias and scale columns in shared memory ([2][BN]).  The activation is a template argument: a runtime
+// switch per element, unrolled over BN / 2 elements, would not fit the instruction cache.  For the same reason GELU and
+// SiLU run a rolled loop over the column groups (the accumulators shift down one group per step), so their erf / exp code
+// appears once.  G column groups per batch: every residual load of a batch is issued before its first use.  With one
+// group per batch (BN = 256, where 128 accumulators leave no room for more, and the rolled loop) each step would wait a
+// full L2 round trip for its residual; prefetch.global.L1 requests the groups PF steps ahead without registers.
+template <int BN, int ACT>
+__device__ __forceinline__ void conv_finish_frag(const ConvTcArgs& a, float* acc, const float* bs, int m0, int n0) {
+    constexpr bool ROLL = ACT == ACT_GELU || ACT == ACT_SILU;
+    constexpr int G = (ROLL || BN == 256) ? 1 : 8, NG = BN / 8, PF = 8;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int r = m0 + (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int c = (lane & 3) * 2;
+    const bool ok[2] = {r < a.M, r + 8 < a.M};
+    auto res_at = [&](int h, int k) { return a.res + (size_t)(r + 8 * h) * a.ldres + n0 + c + 8 * k; };
+    auto prefetch = [&](int k) {
+        if (G == 1 && a.res && k < NG) {
+            if (ok[0]) prefetch_l1(res_at(0, k));
+            if (ok[1]) prefetch_l1(res_at(1, k));
+        }
+    };
+    // one column group: o = act(fmaf(acc, scale, bias) + res), acc[j], acc[j + 1] at row r + 8 h
+    auto group = [&](int k, int h, float a0, float a1, float2 rs) {
+        const int n = c + 8 * k;
+        const float2 b2 = *reinterpret_cast<const float2*>(bs + n), s2 = *reinterpret_cast<const float2*>(bs + BN + n);
+        // o * s is exact (s is a power of two), so the fma rounds like o * s + b
+        float ox = fmaf(a0, s2.x, b2.x), oy = fmaf(a1, s2.y, b2.y);
+        ox += rs.x; oy += rs.y;
+        ox = apply_act(ox, ACT); oy = apply_act(oy, ACT);
+        if (ok[h]) *reinterpret_cast<float2*>(a.out + (size_t)(r + 8 * h) * a.ldout + n0 + n) = make_float2(ox, oy);
+    };
 #pragma unroll
-    for (int b = 0; b < FinishPre<BN>::B; ++b) {
-        const int m = m0 + r0 + b * RSTEP;
-        pre.rs[b] = (a.res && m < a.M) ? *reinterpret_cast<const float4*>(a.res + (size_t)m * a.ldres + n)
-                                       : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-}
-
-template <int BN>
-__device__ __forceinline__ void conv_finish_tile_pre(const ConvTcArgs& a, const uint8_t* smem, int tid, int m0, int n0,
-                                                     const FinishPre<BN>& pre) {
-    constexpr int LD = BN + 4, C4 = BN / 4, RSTEP = 256 / C4, ITERS = 128 / RSTEP, B = FinishPre<BN>::B;
-    static_assert(ITERS % B == 0, "finish tiling");
-    const int c = (tid % C4) * 4, n = n0 + c, r0 = tid / C4;
-    const uint32_t sbase = smem_u32(reinterpret_cast<const float*>(smem) + r0 * LD + c);
-    float4 rs[B];
-#pragma unroll
-    for (int b = 0; b < B; ++b) rs[b] = pre.rs[b];
+    for (int k = 0; k < PF; ++k) prefetch(k);
+    if constexpr (ROLL) {
 #pragma unroll 1
-    for (int i0 = 0; i0 < ITERS; i0 += B) {
-        float4 v[B], nx[B];
+        for (int k = 0; k < NG; ++k) {
+            prefetch(k + PF);
+            float2 rs[2];
 #pragma unroll
-        for (int b = 0; b < B; ++b)
-            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v[b].x), "=f"(v[b].y), "=f"(v[b].z), "=f"(v[b].w)
-                         : "r"(sbase + (uint32_t)((i0 + b) * RSTEP * LD) * 4u));
-        if (i0 + B < ITERS) {                      // residual rows of the next batch, in flight while this one is stored
+            for (int h = 0; h < 2; ++h)
+                rs[h] = (a.res && ok[h]) ? *reinterpret_cast<const float2*>(res_at(h, k)) : make_float2(0.f, 0.f);
 #pragma unroll
-            for (int b = 0; b < B; ++b) {
-                const int m = m0 + r0 + (i0 + B + b) * RSTEP;
-                nx[b] = (a.res && m < a.M) ? *reinterpret_cast<const float4*>(a.res + (size_t)m * a.ldres + n)
-                                           : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
+            for (int h = 0; h < 2; ++h) group(k, h, acc[2 * h], acc[2 * h + 1], rs[h]);
+#pragma unroll
+            for (int i = 0; i < BN / 2 - 4; ++i) acc[i] = acc[i + 4];
         }
+    } else {
 #pragma unroll
-        for (int b = 0; b < B; ++b) {
-            float4 o = v[b];
-            o.x = fmaf(o.x, pre.s4.x, pre.b4.x); o.y = fmaf(o.y, pre.s4.y, pre.b4.y);
-            o.z = fmaf(o.z, pre.s4.z, pre.b4.z); o.w = fmaf(o.w, pre.s4.w, pre.b4.w);
-            o.x += rs[b].x; o.y += rs[b].y; o.z += rs[b].z; o.w += rs[b].w;
-            o.x = apply_act(o.x, a.act); o.y = apply_act(o.y, a.act);
-            o.z = apply_act(o.z, a.act); o.w = apply_act(o.w, a.act);
-            const int m = m0 + r0 + (i0 + b) * RSTEP;
-            if (m < a.M) *reinterpret_cast<float4*>(a.out + (size_t)m * a.ldout + n) = o;
-        }
-        if (i0 + B < ITERS) {
+        for (int k0 = 0; k0 < NG; k0 += G) {
+            prefetch(k0 + PF);
+            float2 rs[G][2];
 #pragma unroll
-            for (int b = 0; b < B; ++b) rs[b] = nx[b];
+            for (int k = 0; k < G; ++k)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    rs[k][h] = (a.res && ok[h]) ? *reinterpret_cast<const float2*>(res_at(h, k0 + k)) : make_float2(0.f, 0.f);
+#pragma unroll
+            for (int k = 0; k < G; ++k)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) group(k0 + k, h, acc[4 * (k0 + k) + 2 * h], acc[4 * (k0 + k) + 2 * h + 1], rs[k][h]);
         }
     }
 }
 
-template <int BN, int STAGES, bool SPLIT>
+template <int BN, int STAGES, bool SPLIT, bool PERSIST>
 struct ConvSmem {
     static constexpr int A_BYTES = CONV_A_BYTES;
     static constexpr int B_BYTES = BN * 128;
     static constexpr int PARTS = SPLIT ? 2 : 1;        // hi and lo tiles, or hi only
     static constexpr int STAGE_BYTES = PARTS * A_BYTES + PARTS * B_BYTES;
-    static constexpr int STG_LD = BN + 4;              // staging tile [128][BN + 4] fp32, aliases the stages
+    static constexpr int STG_LD = BN + 4;              // split-K staging tile [128][BN + 4] fp32, aliases the stages
     static_assert(128 * STG_LD * 4 <= STAGES * STAGE_BYTES, "staging tile must fit in the operand stages");
-    static constexpr int TOTAL = STAGES * STAGE_BYTES + 128 * (int)sizeof(RowInfo) + 3 * STAGES * 8 + 1024;
+    // persistent: row tables of two tiles and the bias / scale columns of two tiles; split-K: one row table
+    static constexpr int RTABLES = PERSIST ? 2 : 1, BS_FLOATS = PERSIST ? 2 * 2 * BN : 0;
+    static constexpr int TOTAL = STAGES * STAGE_BYTES + RTABLES * 128 * (int)sizeof(RowInfo) + BS_FLOATS * 4 + 3 * STAGES * 8 + 1024;
     static_assert(TOTAL <= 227 * 1024, "shared memory of one CTA");
 };
 
-template <int BN, int STAGES, bool SPLIT>
+// PERSIST (launches without split-K): grid.x <= tiles CTAs, CTA b computing tiles b, b + grid.x, ... with t = mb * ntn + nb
+// (the N tiles of one M block are adjacent), the finish straight from the accumulators.  !PERSIST (split-K): grid
+// (M tiles, N tiles, splits), one tile per CTA, the cluster's partial tiles summed through staging tiles.  Separate
+// instantiations, so the split-K launches run a one-tile body without the tile loop and the per-activation finishes.
+template <int BN, int STAGES, bool SPLIT, bool PERSIST>
 __global__ void __launch_bounds__(384, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const ConvTcArgs a) {
-    using SM = ConvSmem<BN, STAGES, SPLIT>;
+    using SM = ConvSmem<BN, STAGES, SPLIT, PERSIST>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    RowInfo* rinfo = reinterpret_cast<RowInfo*>(smem + STAGES * SM::STAGE_BYTES);
-    uint64_t* a_full = reinterpret_cast<uint64_t*>(rinfo + 128);    // 128 producer-thread arrivals
+    RowInfo* rinfo = reinterpret_cast<RowInfo*>(smem + STAGES * SM::STAGE_BYTES);   // [RTABLES][128]: tiles j, j + 1
+    float* bsm = reinterpret_cast<float*>(rinfo + SM::RTABLES * 128);  // [2][2][BN]: bias, scale of tiles j, j + 1
+    uint64_t* a_full = reinterpret_cast<uint64_t*>(bsm + SM::BS_FLOATS);  // 128 producer-thread arrivals
     uint64_t* b_full = a_full + STAGES;                               // TMA transaction bytes
     uint64_t* s_free = b_full + STAGES;                               // 8 consumer-warp arrivals
 
     const int tid = threadIdx.x, warp = tid >> 5;
-    const int m0 = blockIdx.x * 128, n0 = blockIdx.y * BN;
+    const int ntn = a.Cout / BN, ntiles = a.mtiles * ntn;
+    // tiles of this CTA
+    const int ntc = !PERSIST ? 1 : (int)blockIdx.x < ntiles ? (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+    auto tile_m0 = [&](int j) {
+        if constexpr (PERSIST) return ((int)(blockIdx.x + j * gridDim.x) / ntn) * 128;
+        else return (int)blockIdx.x * 128;
+    };
+    auto tile_n0 = [&](int j) {
+        if constexpr (PERSIST) return ((int)(blockIdx.x + j * gridDim.x) % ntn) * BN;
+        else return (int)blockIdx.y * BN;
+    };
     long long* prof = a.prof ? a.prof + 12 * ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
     auto stamp = [&](int slot) { if (prof) prof[slot] = clock64(); };
     if (tid == 0) stamp(0);
     pdl_trigger();      // the next kernel may start its prologue; it waits for this grid before reading our output
 
-    if (tid == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&a_full[s], 128); mbar_init(&b_full[s], 1); mbar_init(&s_free[s], 8); }
-        fence_mbar_init();
-    }
-    if (tid < 128) {
-        const int m = m0 + tid;
+    const int per = PERSIST ? a.nchunks : (a.nchunks + a.splits - 1) / a.splits;
+    const int kbeg = PERSIST ? 0 : blockIdx.z * per;
+    const int nloc = max(0, min(per, a.nchunks - kbeg));     // chunks per tile of this CTA (local it <-> chunk kbeg + it)
+    // Global chunk g = j * nloc + it runs on across the CTA's tiles: stage g % STAGES, phase (g / STAGES) & 1.
+    const int nchk = ntc * nloc;
+    // constant weights (a.const_w): the B tiles of the first STAGES chunks are requested before the grid dependency wait
+    const int npre = a.const_w ? min(STAGES, nchk) : 0;
+    auto issue_b = [&](int g) {
+        const int j = PERSIST ? g / nloc : 0, it = g - j * nloc, s = g % STAGES;
+        uint8_t* Bh = smem + s * SM::STAGE_BYTES + SM::PARTS * SM::A_BYTES;
+        mbar_arrive_expect_tx(&b_full[s], SM::PARTS * SM::B_BYTES);
+        tma_load_2d(Bh, &tmWh, &b_full[s], (kbeg + it) * 64, tile_n0(j));
+        if constexpr (SPLIT) tma_load_2d(Bh + SM::B_BYTES, &tmWl, &b_full[s], (kbeg + it) * 64, tile_n0(j));
+    };
+    // row table of tile j -> rinfo[j & 1], one row per producer thread
+    auto write_rows = [&](int j, int p) {
+        const int m = tile_m0(j) + p;
         RowInfo ri;
         if (m < a.M) {
             const int HoWo = a.Ho * a.Wo;
@@ -240,76 +280,122 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
         } else {
             ri.pix_base = 0; ri.iy0 = 0; ri.ix0 = 0; ri.valid = 0;
         }
-        rinfo[tid] = ri;
+        rinfo[(j & 1) * 128 + p] = ri;
+    };
+
+    if (tid == 0) {
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&a_full[s], 128); mbar_init(&b_full[s], 1); mbar_init(&s_free[s], 8); }
+        fence_mbar_init();
+    }
+    if (tid >= 256) {
+        for (int j = 0; j < min(ntc, 2); ++j) write_rows(j, tid - 256);
     }
     __syncthreads();
     if (tid == 0) stamp(1);
+    if (tid == 256) {
+        tma_prefetch_desc(&tmWh);
+        if constexpr (SPLIT) tma_prefetch_desc(&tmWl);
+        for (int g = 0; g < npre; ++g) issue_b(g);
+    }
     pdl_wait();         // activations / residual below were written by earlier kernels
     const int cpt = (a.Cin % 64 == 0) ? (a.Cin >> 6) : 0;  // 64-wide chunks per filter tap (0: general Cin % 4 path)
-    const int per = (a.nchunks + a.splits - 1) / a.splits;
-    const int kbeg = blockIdx.z * per;
-    const int nloc = max(0, min(per, a.nchunks - kbeg));     // chunks of this CTA (local index it <-> chunk kbeg + it)
 
-    FinishPre<BN> pre;
     // warpgroup index made warp-uniform for the compiler: wgmma in a branch it cannot prove uniform is serialised
     const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
     if (wg < 2) {
-        // ======================= consumers: wgmma only =======================
+        // ======================= consumers: wgmma, then the finish of each tile =======================
         const uint64_t dA0 = smem_desc_sw128(smem_u32(smem + wg * 64 * 128));
         const uint64_t dB0 = smem_desc_sw128(smem_u32(smem + SM::PARTS * SM::A_BYTES));
-        float acc[BN / 2];
-#pragma unroll
-        for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+        int g = 0;
 #pragma unroll 1
-        for (int it = 0; it < nloc; ++it) {
-            const int s = it % STAGES;
-            const uint32_t ph = (it / STAGES) & 1;
-            mbar_wait_cp(&a_full[s], ph, a.spin);
-            mbar_wait_cp(&b_full[s], ph, a.spin);
-            if (it == 0 && tid == 0) stamp(3);
-            const uint64_t so = (uint64_t)((s * SM::STAGE_BYTES) >> 4);
-            const uint64_t ah = dA0 + so, al = ah + (SM::A_BYTES >> 4), bh = dB0 + so, bl = bh + (uint64_t)(SM::B_BYTES >> 4);
-            reg_fence<BN / 2>(acc);
-            wgmma_fence();
+        for (int j = 0; j < ntc; ++j) {
+            float acc[BN / 2];
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-                wgmma_conv<BN>(acc, ah + 2 * ks, bh + 2 * ks);
-                if constexpr (SPLIT) {
-                    wgmma_conv<BN>(acc, al + 2 * ks, bh + 2 * ks);
-                    wgmma_conv<BN>(acc, ah + 2 * ks, bl + 2 * ks);
-                }
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            float* bs = bsm + (j & 1) * 2 * BN;
+            if (PERSIST && tid < BN) {            // read by the finish after the K loop, behind the barrier below
+                const int n = tile_n0(j) + tid;
+                bs[tid] = a.bias ? __ldg(a.bias + n) : 0.f;
+                bs[BN + tid] = a.wscale ? __ldg(a.wscale + n) : 1.f;
             }
-            wgmma_commit();
+#pragma unroll 1
+            for (int it = 0; it < nloc; ++it, ++g) {
+                const int s = g % STAGES;
+                const uint32_t ph = (g / STAGES) & 1;
+                mbar_wait_cp(&a_full[s], ph, a.spin);
+                mbar_wait_cp(&b_full[s], ph, a.spin);
+                if (g == 0 && tid == 0) stamp(3);
+                const uint64_t so = (uint64_t)((s * SM::STAGE_BYTES) >> 4);
+                const uint64_t ah = dA0 + so, al = ah + (SM::A_BYTES >> 4), bh = dB0 + so, bl = bh + (uint64_t)(SM::B_BYTES >> 4);
+                reg_fence<BN / 2>(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks) {
+                    wgmma_conv<BN>(acc, ah + 2 * ks, bh + 2 * ks);
+                    if constexpr (SPLIT) {
+                        wgmma_conv<BN>(acc, al + 2 * ks, bh + 2 * ks);
+                        wgmma_conv<BN>(acc, ah + 2 * ks, bl + 2 * ks);
+                    }
+                }
+                wgmma_commit();
+                reg_fence<BN / 2>(acc);
+                wgmma_wait<1>();                              // the MMAs of the previous chunk have completed: release its stage
+                if (it > 0) mbar_arrive_warp(&s_free[(g - 1) % STAGES]);
+            }
+            wgmma_wait<0>();
             reg_fence<BN / 2>(acc);
-            wgmma_wait<1>();                              // the MMAs of the previous chunk have completed: release its stage
-            if (it > 0) mbar_arrive_warp(&s_free[(it - 1) % STAGES]);
+            if (tid == 0) { if (PERSIST && j == 0) stamp(10); stamp(4); }
+            if constexpr (PERSIST) {
+                if (nloc > 0) mbar_arrive_warp(&s_free[(g - 1) % STAGES]);   // the producer may refill it for the next tile
+                // the bias / scale columns of tile j are visible; every consumer has finished tile j - 1, whose buffer
+                // tile j + 1 rewrites
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                const int m0 = tile_m0(j), n0 = tile_n0(j);
+                switch (a.act) {
+                    case ACT_RELU: conv_finish_frag<BN, ACT_RELU>(a, acc, bs, m0, n0); break;
+                    case ACT_GELU: conv_finish_frag<BN, ACT_GELU>(a, acc, bs, m0, n0); break;
+                    case ACT_SILU: conv_finish_frag<BN, ACT_SILU>(a, acc, bs, m0, n0); break;
+                    case ACT_RELU6: conv_finish_frag<BN, ACT_RELU6>(a, acc, bs, m0, n0); break;
+                    default: conv_finish_frag<BN, ACT_NONE>(a, acc, bs, m0, n0); break;
+                }
+                if (tid == 0) { if (j == 0) stamp(8); stamp(9); }
+            } else {
+                // every MMA of both warpgroups has completed before the staging tile overwrites the operand stages (a split-K
+                // CTA has one tile, so the producer writes nothing after its last chunk)
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                conv_acc_to_staging<BN>(acc, reinterpret_cast<float*>(smem), SM::STG_LD);
+                if (tid == 0) stamp(6);
+            }
         }
-        wgmma_wait<0>();
-        reg_fence<BN / 2>(acc);
-        if (tid == 0) stamp(4);
-        if (a.splits == 1) finish_prefetch<BN>(a, tid, m0, n0, pre);      // bias + first residual rows
-        // every MMA of both warpgroups has completed before the staging tile overwrites the operand stages (the producer
-        // wrote nothing after the last chunk, whose stage the consumers have waited for)
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        conv_acc_to_staging<BN>(acc, reinterpret_cast<float*>(smem), SM::STG_LD);
-        if (tid == 0) stamp(6);
     } else {
         // ======================= producer: activation gather + weight TMA =======================
         // Thread p gathers the 16-byte segment q of rows rsub + 8 i (i = 0..15) of every chunk, in two half chunks (rows
-        // [0, 64) then [64, 128)) of 8 float4.  A ring of three half-chunk buffers keeps the next two in flight.
+        // [0, 64) then [64, 128)) of 8 float4.  A ring of three half-chunk buffers keeps the next two in flight, across tile
+        // boundaries: the next tile's chunks are gathered while the consumers finish this one.
         const int p = tid - 256, q = p & 15, rsub = p >> 4;
         // byte offset of this thread's 8-byte slot in the 128 x 64 half tile (128B swizzle; row & 7 == rsub)
         const uint32_t soff = rsub * 128 + (((q >> 1) ^ rsub) << 4) + ((q & 1) << 3);
         const float4* in4 = reinterpret_cast<const float4*>(a.in);
         // source of row rsub + 8 i for the current filter tap, in float4 units (~0u = zero padding / out of range);
-        // recomputed only when the tap changes (never for 1x1 convs and linears, every Cin/64 chunks for 3x3)
+        // recomputed only when the tap or the tile changes (once per tile for 1x1 convs and linears)
         uint32_t off[16];
         int cur_tap = -1, c4 = 0;
-        if (p == 0) { tma_prefetch_desc(&tmWh); if constexpr (SPLIT) tma_prefetch_desc(&tmWl); }
+        const RowInfo* rows = rinfo;
         auto load_half = [&](int h, auto part_c, float4* v) {
             constexpr int part = decltype(part_c)::value;
             if (part == 0) {
-                const int kc = kbeg + (h >> 1);
+                const int g = h >> 1, j = PERSIST ? g / nloc : 0, it = g - j * nloc;
+                if (PERSIST && it == 0) {   // first chunk of tile j: its row table is rinfo[j & 1]
+                    cur_tap = -1;
+                    rows = rinfo + (j & 1) * 128;
+                    if (j > 0) {
+                        // every producer thread has finished reading the table of tile j - 1, and the table of tile j
+                        // (written at the start of tile j - 1) is visible: tile j + 1 reuses the buffer of tile j - 1
+                        asm volatile("bar.sync 2, 128;" ::: "memory");
+                        if (j + 1 < ntc) write_rows(j + 1, p);
+                    }
+                }
+                const int kc = kbeg + it;
                 int tap, c0;
                 if (cpt > 0) { tap = kc / cpt; c0 = ((kc - tap * cpt) << 6) + q * 4; }       // Cin % 64 == 0
                 else { const int k = kc * 64 + q * 4; tap = k / a.Cin; c0 = k - tap * a.Cin; }  // Cin % 4 == 0 (stem)
@@ -320,7 +406,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
                     const int ky = tap / a.KW, kx = tap - ky * a.KW;
 #pragma unroll
                     for (int i = 0; i < 16; ++i) {
-                        const RowInfo ri = rinfo[rsub + i * 8];
+                        const RowInfo ri = rows[rsub + i * 8];
                         const int iy = ri.iy0 + ky, ix = ri.ix0 + kx;
                         off[i] = (kvalid && ri.valid && iy >= 0 && iy < a.H && ix >= 0 && ix < a.W)
                                      ? (uint32_t)(((size_t)(ri.pix_base + iy * a.W + ix) * a.ldin) >> 2)
@@ -336,16 +422,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
         };
         auto store_half = [&](int h, auto part_c, const float4* v) {
             constexpr int part = decltype(part_c)::value;
-            const int it = h >> 1, s = it % STAGES;
+            const int g = h >> 1, s = g % STAGES;
             uint8_t* stage = smem + s * SM::STAGE_BYTES;
             if (part == 0) {
-                if (it >= STAGES) mbar_wait_cp(&s_free[s], ((it / STAGES) - 1) & 1, a.spin);
-                if (p == 0) {
-                    uint8_t* Bh = stage + SM::PARTS * SM::A_BYTES;
-                    mbar_arrive_expect_tx(&b_full[s], SM::PARTS * SM::B_BYTES);
-                    tma_load_2d(Bh, &tmWh, &b_full[s], (kbeg + it) * 64, n0);
-                    if constexpr (SPLIT) tma_load_2d(Bh + SM::B_BYTES, &tmWl, &b_full[s], (kbeg + it) * 64, n0);
-                }
+                if (g >= STAGES) mbar_wait_cp(&s_free[s], ((g / STAGES) - 1) & 1, a.spin);
+                if (p == 0 && g >= npre) issue_b(g);
             }
             uint8_t* Ah = stage + part * 64 * 128 + soff;
             uint8_t* Al = Ah + SM::A_BYTES;
@@ -369,12 +450,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
             if (part == 1) {
                 fence_proxy_async();      // generic-proxy smem writes -> visible to the tensor core (async proxy)
                 mbar_arrive(&a_full[s]);
-                if (it == 0 && p == 0) stamp(2);
+                if (g == 0 && p == 0) stamp(2);
             }
         };
         using P0 = std::integral_constant<int, 0>;
         using P1 = std::integral_constant<int, 1>;
-        const int nh = 2 * nloc;      // half chunks; h -> buffer h % 3, part h % 2
+        const int nh = 2 * nchk;      // half chunks of all tiles; h -> buffer h % 3, part h % 2
         float4 v0[8], v1[8], v2[8];
         if (nh > 0) { load_half(0, P0{}, v0); load_half(1, P1{}, v1); }
 #pragma unroll 1
@@ -398,24 +479,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
         }
         if (p == 0) stamp(5);
     }
-    // Finish: CTA z of a split-K cluster owns rows [z*128/S, (z+1)*128/S) of the tile and reads that slice of every
-    // peer's staging buffer through distributed shared memory, summing in rank order (deterministic); without split-K
-    // (S = 1) it is the CTA's own buffer.  Then bias / residual / activation and coalesced row stores.  No global
-    // partials, no second kernel.
-    __syncwarp();
-    if (a.splits > 1) cluster_sync_all(); else __syncthreads();
-    if (tid == 0) stamp(8);
-    if (warp < 8) {
-        const int zr = a.splits > 1 ? (int)blockIdx.z : 0;
-        if (a.splits == 1) conv_finish_tile_pre<BN>(a, smem, tid, m0, n0, pre);
-        else if (a.splits == 2) conv_finish_tile<BN, 2, 4>(a, smem, tid, m0, n0, zr);
-        else if (a.splits == 4) conv_finish_tile<BN, 4, 2>(a, smem, tid, m0, n0, zr);
-        else conv_finish_tile<BN, 8, 2>(a, smem, tid, m0, n0, zr);
-    }
-    if (tid == 0) stamp(9);
-    if (a.splits > 1) {
+    if constexpr (!PERSIST) {
+        // Split-K finish: CTA z of the cluster owns rows [z*128/S, (z+1)*128/S) of the tile and reads that slice of every
+        // peer's staging buffer through distributed shared memory, summing in rank order (deterministic).  Then bias /
+        // residual / activation and coalesced row stores.  No global partials, no second kernel.
+        __syncwarp();
+        cluster_sync_all();
+        if (tid == 0) stamp(8);
+        if (warp < 8) {
+            const int zr = (int)blockIdx.z, m0 = tile_m0(0), n0 = tile_n0(0);
+            if (a.splits == 2) conv_finish_tile<BN, 2, 4>(a, smem, tid, m0, n0, zr);
+            else if (a.splits == 4) conv_finish_tile<BN, 4, 2>(a, smem, tid, m0, n0, zr);
+            else conv_finish_tile<BN, 8, 2>(a, smem, tid, m0, n0, zr);
+        }
+        if (tid == 0) stamp(9);
         __syncwarp();
         cluster_sync_all();      // nobody leaves (and frees its shared memory) while a peer may still read it
+    } else if (tid == 0 && prof) {
+        prof[11] = ntc;
     }
     if (tid == 0) stamp(7);
 }
@@ -437,22 +518,44 @@ static int make_tmap_weights(CUtensorMap* out, const void* base, int Kpad, int C
     return AOTB_OK;
 }
 
-template <int BN, int STAGES, bool SPLIT>
-static int launch_conv_tc(const CUtensorMap& th, const CUtensorMap& tl, const ConvTcArgs& a, cudaStream_t st) {
-    constexpr int smem = ConvSmem<BN, STAGES, SPLIT>::TOTAL;
+static int sm_count() {
+    static int n = 0;
+    if (n == 0) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+            n = 132;
+    }
+    return n;
+}
+
+// Without split-K one persistent CTA per SM (at most one per tile, at most the grid cap); split-K: one CTA per tile and K slice.
+static dim3 conv_grid(const ConvTcArgs& a, int BN) {
+    if (a.splits > 1) return dim3(a.mtiles, a.Cout / BN, a.splits);
+    const int cap = g_conv_grid_cap > 0 ? g_conv_grid_cap : sm_count();
+    return dim3(min(a.mtiles * (a.Cout / BN), cap), 1, 1);
+}
+
+template <int BN, int STAGES, bool SPLIT, bool PERSIST>
+static int launch_conv_tc_as(const CUtensorMap& th, const CUtensorMap& tl, const ConvTcArgs& a, cudaStream_t st) {
+    constexpr int smem = ConvSmem<BN, STAGES, SPLIT, PERSIST>::TOTAL;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             smem);
+        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, STAGES, SPLIT, PERSIST>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) {
             set_error("aotb_conv2d_nhwc_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
             return AOTB_ERR_CUDA;
         }
         configured = true;
     }
-    dim3 grid(cdiv(a.M, 128), a.Cout / BN, a.splits);
-    launch_cluster(conv_tc_kernel<BN, STAGES, SPLIT>, dim3(grid), dim3(384), smem, st, a.splits, th, tl, a);
+    launch_cluster(conv_tc_kernel<BN, STAGES, SPLIT, PERSIST>, conv_grid(a, BN), dim3(384), smem, st, a.splits, th, tl, a);
     return check_launch("aotb_conv2d_nhwc_tc");
+}
+
+template <int BN, int STAGES, bool SPLIT>
+static int launch_conv_tc(const CUtensorMap& th, const CUtensorMap& tl, const ConvTcArgs& a, cudaStream_t st) {
+    return a.splits > 1 ? launch_conv_tc_as<BN, STAGES, SPLIT, false>(th, tl, a, st)
+                        : launch_conv_tc_as<BN, STAGES, SPLIT, true>(th, tl, a, st);
 }
 
 }  // namespace tc
@@ -466,6 +569,12 @@ extern "C" int aotb_set_conv_tiling(int mode) {
     return AOTB_OK;
 }
 
+extern "C" int aotb_set_conv_grid_cap(int ctas) {
+    AOTB_REQUIRE(ctas >= 0, "aotb_set_conv_grid_cap: negative cap");
+    tc::g_conv_grid_cap = ctas;
+    return AOTB_OK;
+}
+
 // wh / wl: pre-split weights [Cout][Kpad] fp16 (K = KH*KW*Cin ordered (ky,kx,ci), zero-padded to a multiple of 64);
 // wl == null selects the single-pass kernel (hi operands only); wscale [Cout]: per-channel factor of the accumulator (null = 1).
 extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* wl, const float* bias, const float* wscale,
@@ -474,6 +583,8 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
                                    void* stream) {
     AOTB_REQUIRE(in && wh && out, "aotb_conv2d_nhwc_tc: null pointer");
     const bool split = wl != nullptr;
+    const int const_w = (act & tc::AOTB_CONV_CONST_WEIGHTS) ? 1 : 0;
+    act &= ~tc::AOTB_CONV_CONST_WEIGHTS;
     AOTB_REQUIRE(Cin % 4 == 0 && Cout % 64 == 0, "aotb_conv2d_nhwc_tc: Cin must be a multiple of 4, Cout of 64");
     AOTB_REQUIRE(act >= aotb::ACT_NONE && act <= aotb::ACT_RELU6, "aotb_conv2d_nhwc_tc: activation %d not supported (0-4)", act);
     AOTB_REQUIRE(ldin % 4 == 0 && ldout % 4 == 0 && (!res || ldres % 4 == 0) && ((uintptr_t)in % 16 == 0) &&
@@ -490,14 +601,22 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     AOTB_REQUIRE(a.Ho > 0 && a.Wo > 0, "aotb_conv2d_nhwc_tc: empty output");
     a.Cout = Cout; a.ldout = ldout; a.ldres = ldres; a.KH = KH; a.KW = KW; a.stride = stride; a.pad = pad;
     a.M = B * a.Ho * a.Wo;
+    a.mtiles = cdiv(a.M, 128);
     const int K = ((KH * KW * Cin + 63) / 64) * 64;   // weights are zero-padded to a multiple of 64 along K
     a.nchunks = K / 64;
     a.act = act;
+    a.const_w = const_w;
     // Tile policy: pick the N tile (64 / 128 / 256 dividing Cout) and the split-K cluster size (1 / 2 / 4 / 8) that minimise
-    //     T = waves * (ramp + chunks_per_cta * t_chunk[BN] + t_finish[BN]),   t_chunk[BN] = max(kGather, BN / 64)
+    //     split-K (S > 1, one tile per CTA):  T = waves * (ramp + chunks_per_cta * t_chunk[BN] + t_finish[BN])
+    //     persistent (S = 1, tpc = ceil(tiles / 132) tiles per CTA):
+    //         T = ramp + tpc * chunks * t_chunk[BN] + t_finish[BN] + (tpc - 1) * max(0, chunks * t_mma[BN] + t_finish[BN] - chunks * t_chunk[BN])
+    //     t_chunk[BN] = max(kGather, t_mma[BN]),  t_mma[BN] = BN / 64
     // over the 132 SMs of an H100 (one CTA per SM).  Costs are in units of the MMAs of one BN = 64 chunk.  The producer's
     // gather of a chunk (32 KB of fp32 activations) overlaps the MMAs and takes kGather units whatever BN is, so narrow
-    // tiles are gather-bound and BN = 256 is MMA-bound.  Split-K is only used to fill a partial wave.  kGather was fitted
+    // tiles are gather-bound and BN = 256 is MMA-bound.  A persistent CTA pays the ramp once, and the finish of a tile runs
+    // while the producer gathers the next tile, so only the part of the consumers' MMAs + finish that exceeds the gather of a
+    // tile is added per further tile (the last tile's finish is never hidden).  Split-K is only used to fill a partial wave.
+    // kGather was fitted
     // with scripts/conv_sweep.py on an H100 (80GB HBM3, 700 W): over the 20 conv / linear shapes of an R50-AOTL 480p frame
     // the policy's tiles take 632 us in total against 632 us for the best measured tiling of each shape.  Bit 0 of the
     // tuning mask ("narrow") selects the simpler heuristic instead.
@@ -505,24 +624,33 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     // kGather1 (half the shared-memory stores, no lo split), so every tile is gather-bound and the choice turns on waves
     // and finish cost.  Checked with scripts/conv_sweep.py --single-pass on the same card and shapes: the policy's tiles
     // take 478 us against 473 us for the best measured tiling of each shape (the split kernel's policy: 633 us).
+    // After the persistent schedule, over the 22 shapes of the sweep (the stem and layer 2's first 1x1 added), the policy's
+    // tiles take 664 us (fp32) and 509 us (fp16) against 753 / 582 us before; the split-K picks were left as they were.
     const int mt = cdiv(a.M, 128);
     int BN = 64, best_s = 1;
     const float kGather = 2.5f, kGather1 = 2.0f;
     if ((tc::g_conv_tiling & 1) == 0) {
         float best = 1e30f;
         const int bns[3] = {256, 128, 64};
-        const float t_chunk[3] = {fmaxf(kGather, 4.0f), fmaxf(kGather, 2.0f), fmaxf(kGather, 1.0f)};
-        const float t_chunk1[3] = {fmaxf(kGather1, 4.0f / 3), fmaxf(kGather1, 2.0f / 3), fmaxf(kGather1, 1.0f / 3)};
+        const float t_mma[3] = {4.0f, 2.0f, 1.0f}, t_mma1[3] = {4.0f / 3, 2.0f / 3, 1.0f / 3};
         const float t_fin[3] = {8.0f, 4.0f, 2.0f};
         for (int bi = 0; bi < 3; ++bi) {
+            // beside 128 accumulator registers the BN = 256 finish reads the residual one column group at a time
+            const float tf = t_fin[bi] * (bi == 0 && res ? 2.0f : 1.0f);
             if (Cout % bns[bi]) continue;
+            const float tm = split ? t_mma[bi] : t_mma1[bi], tc = fmaxf(split ? kGather : kGather1, tm);
             for (int sp = 1; sp <= 8; sp <<= 1) {
                 if (sp > a.nchunks) break;
                 const int ctas = mt * (Cout / bns[bi]) * sp;
                 const int slots = sp == 8 ? 128 : 132;                        // co-resident CTAs with clusters of sp
                 if (sp > 1 && ctas > slots) continue;                         // split-K only to fill a partial wave
-                const int waves = cdiv(ctas, slots);
-                const float t = waves * (3.0f + cdiv(a.nchunks, sp) * (split ? t_chunk[bi] : t_chunk1[bi]) + t_fin[bi]);
+                float t;
+                if (sp == 1) {
+                    const int tpc = cdiv(ctas, 132);
+                    t = 3.0f + tpc * a.nchunks * tc + tf + (tpc - 1) * fmaxf(0.f, a.nchunks * (tm - tc) + tf);
+                } else {
+                    t = cdiv(ctas, slots) * (3.0f + cdiv(a.nchunks, sp) * tc + t_fin[bi]);
+                }
                 if (t < best) { best = t; BN = bns[bi]; best_s = sp; }
             }
         }
@@ -540,7 +668,6 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
         AOTB_REQUIRE((BN == 64 || BN == 128 || BN == 256) && Cout % BN == 0, "aotb_conv2d_nhwc_tc: forced tile %d invalid", BN);
     }
     a.splits = force_bn ? 1 : best_s;
-    const int ctas = mt * (Cout / BN);
     if (force_s) {
         AOTB_REQUIRE((force_s == 1 || force_s == 2 || force_s == 4 || force_s == 8) && force_s <= a.nchunks,
                      "aotb_conv2d_nhwc_tc: forced split %d invalid", force_s);
@@ -549,7 +676,8 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     a.spin = (tc::g_conv_tiling & 2) ? 1 : 0;
     a.prof = nullptr;
     if (tc::g_conv_tiling & 4) {      // diagnostic stamps go to the caller's workspace
-        const size_t need = (size_t)ctas * a.splits * 12 * sizeof(long long);
+        const dim3 grid = tc::conv_grid(a, BN);
+        const size_t need = (size_t)grid.x * grid.y * grid.z * 12 * sizeof(long long);
         AOTB_REQUIRE(workspace && workspace_bytes >= need, "aotb_conv2d_nhwc_tc: profile mode needs %zu workspace bytes", need);
         a.prof = (long long*)workspace;
     }

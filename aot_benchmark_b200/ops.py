@@ -141,13 +141,18 @@ def _pow2(e):
     return ((e + 127) << 23).to(torch.int32).view(torch.float32)
 
 
+# flag in the act argument of aotb_conv2d_nhwc_tc (include/aotb200.h): the weights are never written by a kernel
+CONV_CONST_WEIGHTS = 256
+
 # bench.py's encoder probe saves this flag, sets it False and restores it; no encoder path reads it
 CONV_CHAIN = False
 
 
-def conv2d_tc(x, wh, wl, bias, out, res=None, KH=1, KW=1, stride=1, pad=0, act=ACT_NONE, stream=None, wscale=None):
+def conv2d_tc(x, wh, wl, bias, out, res=None, KH=1, KW=1, stride=1, pad=0, act=ACT_NONE, stream=None, wscale=None,
+              const_w=False):
     """Tensor-core conv: x [B,H,W,Cin] fp32, wh/wl [Cout, KH*KW*Cin] fp16, wscale fp32 [Cout] or None (= 1).
-    wl None: the single-pass kernel (x rounded once to fp16, wh only)."""
+    wl None: the single-pass kernel (x rounded once to fp16, wh only).  const_w: no earlier kernel in the stream writes
+    wh / wl (packed model weights), so the kernel may load them before it waits for the previous kernel."""
     _chk(x, bias, out, res, wscale)
     B, H, W, Cin = x.shape
     Cout = wh.shape[0]
@@ -155,7 +160,8 @@ def conv2d_tc(x, wh, wl, bias, out, res=None, KH=1, KW=1, stride=1, pad=0, act=A
     with _ConvProbe(2.0 * out.shape[0] * out.shape[1] * out.shape[2] * Cout * KH * KW * Cin, stream):
         check(lib().aotb_conv2d_nhwc_tc(_p(x), wh.data_ptr(), _p(wl), _p(bias), _p(wscale), _p(res), _p(out), B, H, W, Cin,
                                         _nhwc_ld(x), Cout, _nhwc_ld(out), _nhwc_ld(res) if res is not None else 0, KH, KW,
-                                        stride, pad, act, ws.data_ptr(), ws.numel(), _st(stream)), "aotb_conv2d_nhwc_tc")
+                                        stride, pad, act | (CONV_CONST_WEIGHTS if const_w else 0), ws.data_ptr(), ws.numel(),
+                                        _st(stream)), "aotb_conv2d_nhwc_tc")
     return out
 
 
@@ -165,7 +171,7 @@ def conv2d(x, w, bias, out, res=None, KH=1, KW=1, stride=1, pad=0, dil=1, act=AC
         t = _TC_WEIGHTS.get(w.data_ptr())
         if t is not None:
             return conv2d_tc(x, t[0], None if _PRECISION == "fp16" else t[1], bias, out, res=res, KH=KH, KW=KW, stride=stride, pad=pad, act=act,
-                             stream=stream, wscale=t[2])
+                             stream=stream, wscale=t[2], const_w=True)
     _chk(x, w, bias, out, res)
     B, H, W, Cin = x.shape
     Cout = w.shape[1]
@@ -188,7 +194,7 @@ def linear(x, wt, bias, out, res=None, act=ACT_NONE, stream=None):
                 wl = None if _PRECISION == "fp16" else t[1]
                 check(lib().aotb_conv2d_nhwc_tc(_p(x), t[0].data_ptr(), _p(wl), _p(bias), _p(t[2]), _p(res), _p(out),
                                                 1, M, 1, K, x.stride(0), N, out.stride(0), res.stride(0) if res is not None else 0,
-                                                1, 1, 1, 0, act, ws.data_ptr(), ws.numel(), _st(stream)),
+                                                1, 1, 1, 0, act | CONV_CONST_WEIGHTS, ws.data_ptr(), ws.numel(), _st(stream)),
                       "aotb_conv2d_nhwc_tc")
             return out
     _chk(x, wt, bias, out, res)
@@ -201,7 +207,8 @@ def linear(x, wt, bias, out, res=None, act=ACT_NONE, stream=None):
 
 def linear_tc(x, wh, wl, bias, out, res=None, act=ACT_NONE, stream=None):
     """out[M][N] = act(x[M][K] @ W^T + bias + res) on the tensor-core GEMM with explicitly given split-fp16 weights
-    wh / wl [N][K] (K % 64 == 0, N % 64 == 0) -- e.g. operand copies of the memory bank."""
+    wh / wl [N][K] (K % 64 == 0, N % 64 == 0) -- e.g. operand copies of the memory bank.  Kernels of the same stream
+    may write wh / wl, so the weights are read only after the previous kernel (CONV_CONST_WEIGHTS stays clear)."""
     _chk(x, bias, out, res)
     if wh.dtype != torch.float16 or wl.dtype != torch.float16 or wh.shape != wl.shape or not wh.is_contiguous() \
             or not wl.is_contiguous():

@@ -30,12 +30,17 @@ void aotb_set_pdl(int on);
  *   bit 0: the pre-cost-model heuristic (N = 64 tiles unless a wider tile fills the GPU on its own) instead of the
  *          fitted cost model over N tile x split-K cluster size;
  *   bit 1: mbarrier waits spin without the suspend hint;
- *   bit 2: every CTA writes clock64 stamps (0 start, 1 prologue done, 2 first A stage stored, 3 first stage
- *          consumable, 4 last MMA issued, 5 accumulator complete, 6 tile staged, 7 exit, 8 tile visible to the
- *          finish (cluster barrier), 9 finish stored, 10-11 unused) to `workspace` as long long[ctas][12];
+ *   bit 2: every CTA writes clock64 stamps to `workspace` as long long[ctas][12]: 0 start, 1 prologue done, 2 first A
+ *          stage stored, 3 first stage consumable, 4 accumulator (of the last tile) complete, 5 producer done, 7 exit;
+ *          split-K launches: 6 tile staged, 8 tile visible to the finish (cluster barrier), 9 finish stored;
+ *          persistent launches: 10 accumulator of the first tile complete, 8 finish of the first tile stored (the first
+ *          tile boundary on the consumer side), 9 finish of the last tile stored, 11 the CTA's tile count (not a clock);
  *   bits 4-7: force the N tile (1 = 64, 2 = 128; 0 = policy); bits 8-11: force the split-K factor
  *          (1, 2, 4, 8; 0 = policy).  Forced values that do not divide the problem are an argument error. */
 int aotb_set_conv_tiling(int mode);
+/* Upper bound on the CTAs of a persistent (split-K free) aotb_conv2d_nhwc_tc launch; 0 (default) = one per SM.  The tile
+ * order is static, so the output does not depend on the cap. */
+int aotb_set_conv_grid_cap(int ctas);
 
 /* nn.Conv2d (+ folded FrozenBatchNorm2d, + residual, + activation) as im2col-free implicit GEMM.
  * networks/encoders/resnet.py:34-54,140-157; networks/layers/normalization.py:30-43;
@@ -61,10 +66,16 @@ int aotb_conv2d_nhwc_f32(const float* in, const float* w, const float* bias, con
  * k-step issues one MMA (Ah Wh) instead of three.  Every product then carries fp16 rounding of both operands (2^-11
  * relative; the weight normalisation still gives any channel scale that precision), accumulated in fp32.  The finish and
  * the range are those of the split kernel; the tile policy has its own cost-model row for it.
+ * act may carry AOTB_CONV_CONST_WEIGHTS: the caller promises that no earlier kernel in the stream (or graph) writes wh / wl,
+ * so the kernel requests its first weight tiles before it waits for the previous kernel (programmatic dependent launch).
+ * Model weights packed once qualify; operand copies that kernels of the same frame refresh (memory-bank keys) do not.
+ * Without split-K the launch is persistent: one CTA per SM walks the 128-pixel x BN output tiles in a static order and
+ * gathers the next tile's operands while it finishes the current one.
  * Requires Cin % 4 == 0 and Cout % 64 == 0.  Few-tile deep-K layers run split-K: the 2 / 4 / 8 CTAs of one output
  * tile form a thread-block cluster and sum their partial tiles over distributed shared memory in rank order
  * (deterministic).  `workspace` / `workspace_bytes` are only used by the diagnostic mode of aotb_set_conv_tiling
  * (may be NULL / 0 otherwise). */
+#define AOTB_CONV_CONST_WEIGHTS 256
 int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* wl, const float* bias, const float* wscale,
                         const float* res, float* out, int B, int H, int W, int Cin, int ldin, int Cout, int ldout, int ldres,
                         int KH, int KW, int stride, int pad, int act, void* workspace, size_t workspace_bytes,

@@ -33,9 +33,11 @@ SHAPES = [  # name, H, W, Cin, Cout, K, stride, pad
     ("lstt linear 1024->256", 1674, 1, 1024, 256, 1, 1, 0),
 ]
 REP = 20
-# stamp slots 1..9: consumer thread 0 except "A0 stored" and "producer done" (producer thread 256)
-NAMES = ["prologue", "A0 stored", "stage0 ready", "acc complete", "producer done", "staged", "exit", "finish start",
-         "finish stored"]
+# stamp slots 1..10 (include/aotb200.h): consumer thread 0 except "A0 stored" and "producer done" (producer thread 256);
+# "staged" is split-K only, "first acc complete" persistent only; slot 8 is the split-K finish start or the persistent
+# first finish stored
+NAMES = ["prologue", "A0 stored", "stage0 ready", "last acc complete", "producer done", "staged", "exit",
+         "finish start / first finish stored", "last finish stored", "first acc complete"]
 
 
 def main():
@@ -78,7 +80,7 @@ def main():
             ops.conv2d_tc(x, wh, wl, b, out, KH=K, KW=K, stride=s, pad=p, act=1)
             torch.cuda.synchronize()
             st8 = ws.view(torch.int64)[: 12 * 4096].view(-1, 12).cpu()
-            st8 = st8[st8[:, 7] != 0][:, :10]
+            st8 = st8[st8[:, 7] != 0][:, :11]
             rel = (st8[:, 1:] - st8[:, :1]).double() / 1965.0      # cycles -> us at 1965 MHz
             rel = torch.where(st8[:, 1:] != 0, rel, torch.full_like(rel, float("nan")))
             med = torch.nanmedian(rel, dim=0).values.tolist()
