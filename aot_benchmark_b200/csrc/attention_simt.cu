@@ -231,10 +231,28 @@ extern "C" int aotb_attention_f32(const float* Q, int ldq, const float* K, int l
 // ---------------------------------------------------------------- split-KV merge (cfg4 row e)
 // O = sum_r exp(m_r - m) O_r / sum_r exp(m_r - m) l_r  with m = max_r m_r  (exact LSE merge)
 namespace aotb {
+// USAGE (aotb_attn_merge_usage_f32): split r is memory slot r, and the merge also adds each slot's attention mass
+// l_r exp(m_r - m) / L over its (query, head) pairs into the usage counters; see the entry point.
+constexpr int MERGE_USAGE_MAX_SLOTS = 32;
+constexpr size_t MERGE_USAGE_HDR = 256;            // launch counter, then the per-CTA slot sums (double [gridDim.x][R])
+struct MergeUsage {
+    float* U;             // [R] += mass / (layers H N)
+    int* A;               // [R] += 1 for every live slot (nullptr: no age tick in this launch)
+    const int* live;      // live rows of the bank
+    int rows;             // rows per slot
+    double scale;         // 1 / (layers H N)
+    unsigned* counter;
+    double* partial;
+};
+
+template <bool USAGE>
 __global__ void attn_merge_kernel(const float* __restrict__ Opart, const float* __restrict__ Mpart,
                                   const float* __restrict__ Lpart, float* __restrict__ O, int R, int N, int H,
-                                  int dv, int ldo) {
+                                  int dv, int ldo, const MergeUsage u) {
     pdl_sync();
+    extern __shared__ float usage_red[];         // USAGE: [R][blockDim.x], thread t's mass sums in column t
+    if (USAGE)
+        for (int r = 0; r < R; ++r) usage_red[r * blockDim.x + threadIdx.x] = 0.f;
     // Opart [R][N][H*dv], Mpart/Lpart [R][H][N]; one thread per 4 channels (dv % 4 == 0): the weights of a (query, head) are
     // computed once per float4 instead of once per scalar (same arithmetic and order per element as the scalar form)
     const int dv4 = dv >> 2;
@@ -256,7 +274,42 @@ __global__ void attn_merge_kernel(const float* __restrict__ Opart, const float* 
         }
         *reinterpret_cast<float4*>(O + (size_t)q * ldo + (size_t)h * dv + c) =
             make_float4(num.x / den, num.y / den, num.z / den, num.w / den);
+        if (USAGE && c == 0) {                       // one thread per (query, head): the slot masses, summing to 1
+            for (int r = 0; r < R; ++r) {
+                const float mr = Mpart[((size_t)r * H + h) * N + q];
+                const float w = (mr == -INFINITY) ? 0.f : expf(mr - m);
+                usage_red[r * blockDim.x + threadIdx.x] += w * Lpart[((size_t)r * H + h) * N + q] / den;
+            }
+        }
     }
+    if (!USAGE) return;
+    // per-CTA slot sums: warp w sums slots w, w + 8, ... over the block's threads in a fixed order
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    for (int r = warp; r < R; r += nwarps) {
+        double a = 0.0;
+        for (int t = lane; t < (int)blockDim.x; t += 32) a += (double)usage_red[r * blockDim.x + t];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+        if (lane == 0) u.partial[(size_t)blockIdx.x * R + r] = a;
+    }
+    __threadfence();
+    __syncthreads();
+    __shared__ unsigned last;
+    if (threadIdx.x == 0) last = atomicAdd(u.counter, 1u) == gridDim.x - 1 ? 1u : 0u;
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    // last CTA: the CTA sums in CTA order, then the counters; the launch counter is left at zero for the next launch
+    const volatile double* pv = u.partial;
+    const int live_slots = u.A ? min(*u.live / u.rows, R) : 0;
+    for (int r = threadIdx.x; r < R; r += blockDim.x) {
+        double a = 0.0;
+        for (int b = 0; b < (int)gridDim.x; ++b) a += pv[(size_t)b * R + r];
+        u.U[r] += (float)(a * u.scale);
+        if (r < live_slots) u.A[r] += 1;
+    }
+    if (threadIdx.x == 0) *u.counter = 0u;
 }
 }  // namespace aotb
 
@@ -305,8 +358,35 @@ extern "C" int aotb_attn_merge_f32(const float* Opart, const float* Mpart, const
     const size_t total = (size_t)N * H * (d_v / 4);
     int g = (int)((total + 255) / 256);
     if (g > 132 * 8) g = 132 * 8;
-    launch(attn_merge_kernel, dim3(g), dim3(256), 0, (cudaStream_t)stream, Opart, Mpart, Lpart, O, R, N, H, d_v, ldo);
+    launch(attn_merge_kernel<false>, dim3(g), dim3(256), 0, (cudaStream_t)stream, Opart, Mpart, Lpart, O, R, N, H, d_v, ldo,
+           MergeUsage{});
     return check_launch("aotb_attn_merge_f32");
+}
+
+extern "C" size_t aotb_attn_merge_usage_workspace_bytes(int R) {
+    return MERGE_USAGE_HDR + (size_t)132 * 8 * (size_t)(R > 0 ? R : 0) * sizeof(double);
+}
+
+extern "C" int aotb_attn_merge_usage_f32(const float* Opart, const float* Mpart, const float* Lpart, float* O, int R, int N,
+                                         int H, int d_v, int ldo, float* U, int* A, const int* live, int rows, int layers,
+                                         void* workspace, void* stream) {
+    AOTB_REQUIRE(Opart && Mpart && Lpart && O && R > 0 && N > 0 && H > 0 && d_v > 0, "aotb_attn_merge_usage_f32: bad args");
+    AOTB_REQUIRE(d_v % 4 == 0 && ldo % 4 == 0 && ((uintptr_t)Opart | (uintptr_t)O) % 16 == 0,
+                 "aotb_attn_merge_usage_f32: d_v, ldo %% 4, 16-byte alignment");
+    AOTB_REQUIRE(R <= MERGE_USAGE_MAX_SLOTS, "aotb_attn_merge_usage_f32: at most %d slots (got %d)", MERGE_USAGE_MAX_SLOTS, R);
+    AOTB_REQUIRE(U && workspace && layers > 0 && (!A || (live && rows > 0)), "aotb_attn_merge_usage_f32: usage arguments");
+    AOTB_REQUIRE((uintptr_t)workspace % 16 == 0, "aotb_attn_merge_usage_f32: workspace alignment");
+    const size_t total = (size_t)N * H * (d_v / 4);
+    int g = (int)((total + 255) / 256);
+    if (g > 132 * 8) g = 132 * 8;
+    MergeUsage u;
+    u.U = U; u.A = A; u.live = live; u.rows = rows;
+    u.scale = 1.0 / ((double)layers * H * N);
+    u.counter = (unsigned*)workspace;
+    u.partial = (double*)((char*)workspace + MERGE_USAGE_HDR);
+    launch(attn_merge_kernel<true>, dim3(g), dim3(256), (size_t)R * 256 * sizeof(float), (cudaStream_t)stream, Opart, Mpart,
+           Lpart, O, R, N, H, d_v, ldo, u);
+    return check_launch("aotb_attn_merge_usage_f32");
 }
 
 extern "C" int aotb_attn_merge_peers_f32(const void* const* Oparts, const void* const* Mparts, const void* const* Lparts,

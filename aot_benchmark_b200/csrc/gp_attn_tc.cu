@@ -41,3 +41,29 @@ extern "C" int aotb_gp_attn_tc_f16x2(const void* Qp, int Nq_cap, const void* Kp,
     return tc::launch_attn_tc<4, tc::GP_VC, tc::GP_STAGES, 64, 2, false>(tq, tk, tv, a, dim3(cdiv(N, 128), dv / (32 * tc::GP_VC), splits),
                                                            exact & 1, (cudaStream_t)stream, "aotb_gp_attn_tc_f16x2");
 }
+
+// The same attention over a bounded bank cut into its memory slots: split z = keys [z split_rows, (z + 1) split_rows) of the
+// live ones (see aotb_lt_attn_tc_slots_f16x2).
+extern "C" int aotb_gp_attn_tc_slots_f16x2(const void* Qp, int Nq_cap, const void* Kp, const void* Vp, int kv_cap, int N,
+                                           int Tk, const int* Tk_dev, int dv, float* Opart, float* Mpart, float* Lpart,
+                                           int splits, int split_rows, int exact, void* stream) {
+    AOTB_REQUIRE(Qp && Kp && Vp && N > 0 && (Tk > 0 || Tk_dev) && splits >= 2 && split_rows > 0 && dv > 0 && dv % 128 == 0,
+                 "aotb_gp_attn_tc_slots_f16x2: bad args");
+    AOTB_REQUIRE(Opart && Mpart && Lpart, "aotb_gp_attn_tc_slots_f16x2: output buffers");
+    AOTB_REQUIRE(Tk_dev || Tk <= (long long)splits * split_rows, "aotb_gp_attn_tc_slots_f16x2: more keys than slots");
+    AOTB_REQUIRE((exact & ~5) == 0, "aotb_gp_attn_tc_slots_f16x2: exact bits 0 and 2 only");
+    AOTB_REQUIRE(Nq_cap >= ((N + 127) / 128) * 128, "aotb_gp_attn_tc_slots_f16x2: Q buffer must be padded to 128 rows");
+    AOTB_REQUIRE(((uintptr_t)Qp | (uintptr_t)Kp | (uintptr_t)Vp) % 128 == 0, "aotb_gp_attn_tc_slots_f16x2: alignment");
+    CUtensorMap tq, tk, tv;
+    int rc;
+    if ((rc = tc::make_tmap_rows64(&tq, Qp, Nq_cap, 4, 128)) != AOTB_OK) return rc;
+    if ((rc = tc::make_tmap_rows64(&tk, Kp, kv_cap, 4, 64)) != AOTB_OK) return rc;
+    if ((rc = tc::make_tmap_rows64(&tv, Vp, kv_cap, dv / 32, 64)) != AOTB_OK) return rc;
+    tc::AttnTcArgs a;
+    a.N = N; a.Tk = Tk; a.Tk_dev = Tk_dev; a.O = nullptr; a.ldo = 0;
+    a.Opart = Opart; a.Mpart = Mpart; a.Lpart = Lpart; a.splits = splits; a.split_unit = split_rows;
+    a.spin = (exact >> 2) & 1; a.dbg = nullptr;
+    return tc::launch_attn_tc<4, tc::GP_VC, tc::GP_STAGES, 64, 2, false>(
+        tq, tk, tv, a, dim3(cdiv(N, 128), dv / (32 * tc::GP_VC), splits), exact & 1, (cudaStream_t)stream,
+        "aotb_gp_attn_tc_slots_f16x2");
+}

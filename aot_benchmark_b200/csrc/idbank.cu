@@ -453,6 +453,26 @@ __global__ void ring_advance_kernel(int* live, int* write, int rows, int cap_row
     *write = w;
 }
 
+// Usage policy of the bounded bank, before a store: the next free slot while the bank is not full, else the unpinned slot
+// with the lowest mean attention mass U / A (A == 0 counts as +inf, ties go to the lowest slot); that slot's counters restart.
+__global__ void ring_select_usage_kernel(const int* live, int* write, float* U, int* A, int rows, int cap_rows,
+                                         int pinned_rows) {
+    pdl_sync();
+    const int slots = cap_rows / rows, used = max(*live, 0) / rows;
+    int s = used;
+    if (used >= slots) {
+        float best = 0.f;
+        s = -1;
+        for (int c = pinned_rows / rows; c < slots; ++c) {
+            const float score = A[c] > 0 ? U[c] / (float)A[c] : INFINITY;
+            if (s < 0 || score < best) { s = c; best = score; }
+        }
+    }
+    *write = s * rows;
+    U[s] = 0.f;
+    A[s] = 0;
+}
+
 }  // namespace aotb
 
 using namespace aotb;
@@ -627,4 +647,15 @@ extern "C" int aotb_ring_advance(int* live, int* write, int rows, int cap_rows, 
                  "(got rows %d, cap_rows %d, pinned_rows %d)", rows, cap_rows, pinned_rows);
     launch(ring_advance_kernel, dim3(1), dim3(1), 0, (cudaStream_t)stream, live, write, rows, cap_rows, pinned_rows);
     return check_launch("aotb_ring_advance");
+}
+
+extern "C" int aotb_ring_select_usage(const int* live, int* write, float* U, int* A, int rows, int cap_rows, int pinned_rows,
+                                      void* stream) {
+    AOTB_REQUIRE(live && write && U && A, "aotb_ring_select_usage: null pointer");
+    AOTB_REQUIRE(rows > 0 && pinned_rows >= 0 && pinned_rows % rows == 0 && cap_rows % rows == 0 &&
+                     pinned_rows + rows <= cap_rows,
+                 "aotb_ring_select_usage: need rows > 0, pinned_rows and cap_rows multiples of rows and pinned_rows + rows <= "
+                 "cap_rows (rows %d, cap_rows %d, pinned_rows %d)", rows, cap_rows, pinned_rows);
+    launch(ring_select_usage_kernel, dim3(1), dim3(1), 0, (cudaStream_t)stream, live, write, U, A, rows, cap_rows, pinned_rows);
+    return check_launch("aotb_ring_select_usage");
 }

@@ -130,3 +130,29 @@ extern "C" int aotb_lt_attn_tc_f16x2(const void* Qp, int Nq_cap, const void* Kp,
     if (pair) return tc::launch_attn_tc<1, 1, tc::LT_STAGES, 64, 1, false>(tq, tk, tv, a, grid, exact & 1, st, what);
     return tc::launch_attn_tc<1, 1, tc::LT_STAGES, 64, 2, false>(tq, tk, tv, a, grid, exact & 1, st, what);
 }
+
+// The long-term attention over a bounded bank cut into its memory slots: split z = keys [z split_rows, (z + 1) split_rows)
+// of the live ones, so each split's partial (m, l, O) is slot z's.  Default ("tile") layout only; the exact bits are those
+// of aotb_lt_attn_tc_f16x2 (bit 0 exact, bit 2 spin) and a layout bit is refused.
+extern "C" int aotb_lt_attn_tc_slots_f16x2(const void* Qp, int Nq_cap, const void* Kp, const void* Vp, int kv_cap, int N,
+                                           int Tk, const int* Tk_dev, int H, float* Opart, float* Mpart, float* Lpart,
+                                           int splits, int split_rows, int exact, void* stream) {
+    AOTB_REQUIRE(Qp && Kp && Vp && N > 0 && H > 0 && (Tk > 0 || Tk_dev) && splits >= 2 && split_rows > 0,
+                 "aotb_lt_attn_tc_slots_f16x2: bad args");
+    AOTB_REQUIRE(Opart && Mpart && Lpart, "aotb_lt_attn_tc_slots_f16x2: output buffers");
+    AOTB_REQUIRE(Tk_dev || Tk <= (long long)splits * split_rows, "aotb_lt_attn_tc_slots_f16x2: more keys than slots");
+    AOTB_REQUIRE((exact & ~5) == 0, "aotb_lt_attn_tc_slots_f16x2: only the default layout (exact bits 0 and 2)");
+    AOTB_REQUIRE(Nq_cap >= ((N + 255) / 256) * 256, "aotb_lt_attn_tc_slots_f16x2: Q buffer must be padded to 256 rows");
+    AOTB_REQUIRE(((uintptr_t)Qp | (uintptr_t)Kp | (uintptr_t)Vp) % 128 == 0, "aotb_lt_attn_tc_slots_f16x2: alignment");
+    CUtensorMap tq, tk, tv;
+    int rc;
+    if ((rc = tc::make_tmap_rows64(&tq, Qp, Nq_cap, H, 128)) != AOTB_OK) return rc;
+    if ((rc = tc::make_tmap_rows64(&tk, Kp, kv_cap, H, 64)) != AOTB_OK) return rc;
+    if ((rc = tc::make_tmap_rows64(&tv, Vp, kv_cap, H, 64)) != AOTB_OK) return rc;
+    tc::AttnTcArgs a;
+    a.N = N; a.Tk = Tk; a.Tk_dev = Tk_dev; a.O = nullptr; a.ldo = 0;
+    a.Opart = Opart; a.Mpart = Mpart; a.Lpart = Lpart; a.splits = splits; a.split_unit = split_rows;
+    a.spin = (exact >> 2) & 1; a.dbg = nullptr;
+    return tc::launch_attn_tc<1, 1, tc::LT_STAGES, 64, 2, false>(tq, tk, tv, a, dim3(cdiv(N, 128), H, splits), exact & 1,
+                                                                 (cudaStream_t)stream, "aotb_lt_attn_tc_slots_f16x2");
+}

@@ -8,7 +8,8 @@ and tools/demo.py drive it unedited.  Differences are internal:
 * activations live in NHWC / token-major fp32 buffers allocated once per video;
 * the long-term memory is a pre-allocated append buffer (bank) instead of torch.cat'ed tensors
   (new frames are appended, not prepended -- attention is permutation invariant over keys); with long_term_mem_max = M it
-  holds the first memory frame and the newest M - 1 in a ring, so a long clip runs at constant cost;
+  holds the first memory frame and the newest M - 1 in a ring (with long_term_mem_policy="usage", a full bank overwrites
+  the least-attended unpinned frame instead of the oldest), so a long clip runs at constant cost;
 * every FLOP of the per-frame path runs in libaotb200.so; there is no eager fallback and the
   engines refuse CPU tensors.
 
@@ -106,6 +107,40 @@ def _resolve_mem_max(aot_model, long_term_mem_max):
     if int(m) != m or m < 2:
         raise ValueError(f"long_term_mem_max must be an integer >= 2 (the first memory frame and at least one recent one), got {m}")
     return int(m)
+
+
+MEM_POLICIES = ("fifo", "usage")
+USAGE_MAX_SLOTS = 32          # aotb_attn_merge_usage_f32 counts at most 32 memory slots
+
+
+def _resolve_mem_policy(aot_model, policy, mem_max):
+    """The eviction policy of the bounded bank: the keyword, else cfg.TEST_LONG_TERM_MEM_POLICY, else "fifo".  "fifo" overwrites
+    the oldest unpinned memory frame; "usage" the unpinned frame the propagated frames attended to least on average since it
+    was stored (DESIGN §2).  Usage mode counts attention mass in the tensor-core long-term attention's slot-split launch, so
+    it refuses the knobs that select another kernel."""
+    p = getattr(aot_model.cfg, "TEST_LONG_TERM_MEM_POLICY", None) if policy is None else policy
+    if p is None:
+        return "fifo"
+    if p not in MEM_POLICIES:
+        raise ValueError(f"long_term_mem_policy must be one of {MEM_POLICIES}, got {p!r}")
+    if p == "usage":
+        if mem_max is None:
+            raise ValueError("long_term_mem_policy='usage' chooses which frame a full bounded bank evicts; it needs "
+                             "long_term_mem_max (or cfg.TEST_LONG_TERM_MEM_MAX)")
+        if mem_max > USAGE_MAX_SLOTS:
+            raise NotImplementedError(f"long_term_mem_policy='usage' counts at most {USAGE_MAX_SLOTS} memory slots, "
+                                      f"got long_term_mem_max={mem_max}")
+        if aot_model.cfg.MODEL_VOS == "deaot":
+            if DEAOT_LT != "tc":
+                raise NotImplementedError(f"long_term_mem_policy='usage' counts attention mass in DeAOT's fused tensor-core "
+                                          f"attention; AOTB_DEAOT_LT={DEAOT_LT} selects another path")
+        elif LT_IMPL == "simt":
+            raise NotImplementedError("long_term_mem_policy='usage' counts attention mass in the tensor-core long-term "
+                                      "attention; AOTB_LT_IMPL=simt selects the fp32 CUDA-core kernel")
+        elif ops.LT_VARIANT != "tile":
+            raise NotImplementedError(f"long_term_mem_policy='usage' runs the default 'tile' layout of the tensor-core "
+                                      f"long-term attention; AOTB_LT_VARIANT={ops.LT_VARIANT} selects another")
+    return p
 
 
 def _resolve_precision(aot_model, precision):
@@ -503,10 +538,13 @@ class _Encoder:
 # =====================================================================================
 class AOTEngine(nn.Module):
     def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1, long_term_mem_max=None,
-                 precision=None):
+                 precision=None, long_term_mem_policy=None):
         """long_term_mem_max = M bounds the long-term bank to M memory frames: the first frame stored after
         restart_engine() stays, the other M - 1 slots hold the newest stored frames (the oldest is overwritten).  None: the
         bound of cfg.TEST_LONG_TERM_MEM_MAX if the config has one, else the reference's ever-growing memory.
+        long_term_mem_policy: which frame a full bounded bank overwrites -- "fifo" (default) the oldest, "usage" the one
+        with the lowest mean attention mass since it was stored (see long_term_memory_usage).  None: cfg.TEST_LONG_TERM_MEM_POLICY
+        if the config has one, else "fifo".
         precision: "fp32" (default; split-fp16 tensor-core operands, fp32-faithful) or "fp16" (operands of every
         tensor-core conv, linear and attention product rounded once to fp16, accumulated in fp32).  None: cfg.TEST_PRECISION
         if the config has one, else "fp32"."""
@@ -520,6 +558,7 @@ class AOTEngine(nn.Module):
         self.long_term_mem_gap = long_term_mem_gap
         self.short_term_mem_skip = short_term_mem_skip
         self.long_term_mem_max = _resolve_mem_max(aot_model, long_term_mem_max)
+        self.long_term_mem_policy = _resolve_mem_policy(aot_model, long_term_mem_policy, self.long_term_mem_max)
         self.losses = None
         self._enc = None
         self._ws = None
@@ -559,6 +598,15 @@ class AOTEngine(nn.Module):
         if self.tk_dev is not None:
             self.tk_dev.zero_()
             self.wr_dev.zero_()
+        self._zero_usage()
+
+    def _zero_usage(self):
+        if getattr(self._ws, "usage_U", None) is not None:
+            self._ws.usage_U.zero_()
+            self._ws.usage_A.zero_()
+
+    def _usage(self):
+        return self.long_term_mem_policy == "usage" and self.long_term_mem_max is not None
 
     def enable_kv_sharding(self, rank, world, group=None):
         """BASELINE config 4: shard the long-term bank by memory frame round-robin over `world` ranks.  Every rank
@@ -599,12 +647,14 @@ class AOTEngine(nn.Module):
         if M is not None and P.deaot and DEAOT_LT == "gemm":
             raise NotImplementedError("a bounded long-term bank (long_term_mem_max) is not built for AOTB_DEAOT_LT=gemm: its "
                                       "transposed value copies have no ring store; use the default fused kernel")
-        key = (id(P), N, tuple(self.enc_size_2d), tuple(self.input_size_2d), LT_IMPL, DEAOT_LT, M)
+        usage = self._usage()
+        key = (id(P), N, tuple(self.enc_size_2d), tuple(self.input_size_2d), LT_IMPL, DEAOT_LT, M, usage)
         if self._ws is not None and self._ws_key == key:
             # same geometry and weights as the previous video: keep buffers and captured graphs
             self.bank_len = 0
             self.tk_dev.zero_()
             self.wr_dev.zero_()
+            self._zero_usage()
             self._st_ring = []
             return
         self._ws_key = key
@@ -684,6 +734,17 @@ class AOTEngine(nn.Module):
             self.bank_Kp = [hz(P.H, cap, 64) for _ in range(L)]     # split-fp16 copies read by TMA
             self.bank_Vp = [hz(P.H, cap, 64) for _ in range(L)]
             ws.part = {}
+        if usage:
+            if not (self._tc or self._gp_tc):
+                raise NotImplementedError("long_term_mem_policy='usage' needs the tensor-core long-term attention, which "
+                                          f"this model's head shape ({P.H} x {C // P.H}) does not run on")
+            # per memory slot: summed mean attention mass U and propagated frames since the store A (restart_engine zeroes
+            # both), the merge's CTA sums, and one split of partials per slot
+            ws.usage_U = torch.zeros(M, dtype=torch.float32, device=dev)
+            ws.usage_A = torch.zeros(M, dtype=torch.int32, device=dev)
+            ws.usage_ws = ops.attn_merge_usage_workspace(M, dev)
+            H, dv = (1, self._vdim) if P.deaot else (P.H, C)
+            ws.usage_part = (f(M, N, dv), f(M, H, N), f(M, H, N))
         self._st_ring = []
         self._ws = ws
         self._dec_bufs = {}
@@ -758,6 +819,16 @@ class AOTEngine(nn.Module):
             else:
                 out.append([K, V.unsqueeze(1)])
         return out
+
+    @property
+    def long_term_memory_usage(self):
+        """long_term_mem_policy="usage": (U, A), float32 and int32 [long_term_mem_max], per memory slot (the slot order of
+        long_term_memories): U = the summed per-frame mean attention mass the propagated frames put on the slot's keys, A =
+        frames propagated since the slot was stored; the bank evicts the unpinned slot with the lowest U / A.  Slot 0 is never
+        evicted.  None in FIFO mode or before the first reference frame."""
+        if not self._usage() or getattr(self._ws, "usage_U", None) is None:
+            return None
+        return self._ws.usage_U.clone(), self._ws.usage_A.clone()
 
     @property
     def short_term_memories(self):
@@ -873,6 +944,8 @@ class AOTEngine(nn.Module):
         splits = lt_splits(self.enc_hw, self._plan().H, max(self.bank_len, 1)) if getattr(self, "_tc", False) else 0
         if getattr(self, "_gp_tc", False):
             splits = self._gp_splits(self.bank_len)       # the fused DeAOT kernel's split count is part of the captured body
+        if self._usage():
+            splits = "usage"                              # one split per memory slot, whatever the live count
         if self.kv_shard is not None:
             # sharded bank: the captured body also depends on the shard split count (a function of the GLOBAL memory-frame
             # count, identical on every rank) and on whether this rank holds any memory frame yet
@@ -934,6 +1007,9 @@ class AOTEngine(nn.Module):
             # bounded: one launch per layer writes the fp32 rows and the packed rows of the selected attention kernel at the
             # ring's write offset, then both counters move (the first frame's slot is never the wrap target)
             packed = (self.bank_Kp, self.bank_Vp) if self._tc else (self.bank_gpK, self.bank_gpV) if self._gp_tc else None
+            if self._usage():          # the write offset becomes the next free slot, or the least-attended unpinned one
+                ops.ring_select_usage(self.tk_dev, self.wr_dev, self._ws.usage_U, self._ws.usage_A, N, self.bank_cap, N,
+                                      stream=st)
             for li in range(self._plan().L):
                 ops.bank_ring_store(K_src[li], V_src[li], self.bank_K[li], self.bank_V[li],
                                     packed[0][li] if packed else None, packed[1][li] if packed else None, self.wr_dev, stream=st)
@@ -1031,6 +1107,8 @@ class AOTEngine(nn.Module):
         elif self.kv_shard is not None and K is self.bank_K[li]:
             raise ops.AotbError("sharded long-term bank needs the tensor-core attention kernel (8 heads x 32); this model's "
                                 "head shape runs on the fp32 kernel, which has no partial (m, l, O) outputs")
+        elif use_tc and self._usage():
+            self._usage_attention(li, self._ws.Qp, self.bank_Kp[li], self.bank_Vp[li], out, st)
         elif use_tc:
             self._tc_attention(None, None, None, self.bank_Kp[li], self.bank_Vp[li], Tk, out, st, Tk_dev=self.tk_dev)
         elif self._tc:
@@ -1065,6 +1143,23 @@ class AOTEngine(nn.Module):
                 ws.part[splits] = part
         exact = LT_IMPL == "tc_exact" and self.precision == "fp32"
         ops.lt_attention_tc(ws.Qp, Kp, Vp, N, Tk, O=out, Tk_dev=Tk_dev, splits=splits, exact=exact, part=part, stream=st)
+
+    def _usage_attention(self, li, Qp, Kp, Vp, out, st):
+        """Usage mode: the long-term attention over the bank with one KV split per memory slot (packed Q given), merged by
+        the kernel that also adds each slot's attention mass to U; layer 0's merge ticks A for the live slots."""
+        P = self._plan()
+        ws = self._ws
+        M, N = self.long_term_mem_max, self.enc_hw
+        if P.deaot:
+            H = 1
+            ops.gp_attention_tc_slots(Qp, Kp, Vp, N, self.tk_dev, M, N, ws.usage_part, exact=self.precision == "fp32",
+                                      stream=st)
+        else:
+            H = P.H
+            ops.lt_attention_tc_slots(Qp, Kp, Vp, N, self.tk_dev, M, N, ws.usage_part,
+                                      exact=LT_IMPL == "tc_exact" and self.precision == "fp32", stream=st)
+        ops.attn_merge_usage(*ws.usage_part, out, H, out.shape[1] // H, ws.usage_U, ws.usage_A if li == 0 else None,
+                             self.tk_dev, N, P.L, ws.usage_ws, stream=st)
 
     def _shard_splits(self):
         """KV-split count of the per-rank partial attention in sharded mode: a function of the GLOBAL memory-frame count, so it
@@ -1262,9 +1357,9 @@ class DeAOTEngine(AOTEngine):
     """networks/engines/deaot_engine.py:9-56 -- GatedPropagationModule stack (transformer.py:501-665)."""
 
     def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1,
-                 layer_loss_scaling_ratio=2., long_term_mem_max=None, precision=None):
+                 layer_loss_scaling_ratio=2., long_term_mem_max=None, precision=None, long_term_mem_policy=None):
         super().__init__(aot_model, gpu_id, long_term_mem_gap, short_term_mem_skip, long_term_mem_max=long_term_mem_max,
-                         precision=precision)
+                         precision=precision, long_term_mem_policy=long_term_mem_policy)
         self.layer_loss_scaling_ratio = layer_loss_scaling_ratio
 
     def _gated_tail(self, core, U, dw_w, out_slice, h, w, st):
@@ -1317,7 +1412,10 @@ class DeAOTEngine(AOTEngine):
             if probe is not None:
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record()
-            if self._gp_tc and not is_ref:
+            if self._gp_tc and not is_ref and self._usage():
+                ops.tc_pack_rows(cQ, ws.gpQp, 0, div=math.sqrt(self._kdim), stream=st)
+                self._usage_attention(li, ws.gpQp, self.bank_gpK[li], self.bank_gpV[li], ws.core, st)
+            elif self._gp_tc and not is_ref:
                 # fused wgmma kernel (gp_attn_tc.cu): 128 queries x 64 value channels per CTA, KV splits to fill the GPU
                 self._gp_attention(cQ, None, None, self.bank_gpK[li], self.bank_gpV[li], Tk, self.tk_dev, ws.core, st)
             elif self._gp_tc:
@@ -1420,9 +1518,9 @@ class AOTInferEngine(nn.Module):
     _engine_cls = AOTEngine
 
     def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1, max_aot_obj_num=None,
-                 long_term_mem_max=None, precision=None):
-        """long_term_mem_max: bound of every sub-engine's long-term bank in memory frames; precision: "fp32" | "fp16" of
-        every sub-engine (see AOTEngine for both)."""
+                 long_term_mem_max=None, precision=None, long_term_mem_policy=None):
+        """long_term_mem_max: bound of every sub-engine's long-term bank in memory frames; precision: "fp32" | "fp16" and
+        long_term_mem_policy: "fifo" | "usage" of every sub-engine (see AOTEngine for all three)."""
         super().__init__()
         self.precision = _resolve_precision(aot_model, precision)
         self.cfg = aot_model.cfg
@@ -1435,6 +1533,7 @@ class AOTInferEngine(nn.Module):
         self.long_term_mem_gap = long_term_mem_gap
         self.short_term_mem_skip = short_term_mem_skip
         self.long_term_mem_max = _resolve_mem_max(aot_model, long_term_mem_max)
+        self.long_term_mem_policy = _resolve_mem_policy(aot_model, long_term_mem_policy, self.long_term_mem_max)
         self.aot_engines = []
         self._kv_shard = None
         self.restart_engine()
@@ -1510,8 +1609,10 @@ class AOTInferEngine(nn.Module):
             eng = self._pool.pop(0) if self._pool else self._engine_cls(self.AOT, self.gpu_id, self.long_term_mem_gap,
                                                                        self.short_term_mem_skip,
                                                                        long_term_mem_max=self.long_term_mem_max,
-                                                                       precision=self.precision)
+                                                                       precision=self.precision,
+                                                                       long_term_mem_policy=self.long_term_mem_policy)
             eng.long_term_mem_max = self.long_term_mem_max      # pooled engines too: part of their workspace key
+            eng.long_term_mem_policy = self.long_term_mem_policy
             eng.restart_engine()
             eng.eval()
             if self._kv_shard is not None:
@@ -1554,6 +1655,11 @@ class AOTInferEngine(nn.Module):
     @property
     def pred_id_logits(self):
         return self.aot_engines[0].pred_id_logits if self.aot_engines else None
+
+    @property
+    def long_term_memory_usage(self):
+        """Every sub-engine's long_term_memory_usage (see AOTEngine), in sub-engine order."""
+        return [e.long_term_memory_usage for e in self.aot_engines]
 
 
 class DeAOTInferEngine(AOTInferEngine):

@@ -457,6 +457,28 @@ def attn_merge(Opart, Mpart, Lpart, O, H, d_v, stream=None):
     return O
 
 
+def attn_merge_usage_workspace(R, device):
+    """Zero-filled workspace of attn_merge_usage for up to R slots (its launch counter must start at zero)."""
+    n = int(lib().aotb_attn_merge_usage_workspace_bytes(int(R)))
+    return torch.zeros((n + 7) // 8, dtype=torch.float64, device=device)
+
+
+def attn_merge_usage(Opart, Mpart, Lpart, O, H, d_v, U, A, live_dev, rows, layers, workspace, stream=None):
+    """attn_merge over the R memory slots of a bounded bank (split r = slot r) that also adds each slot's attention mass,
+    averaged over (query, head) and divided by `layers`, into U (float32 [R]); A (int32 [R] or None) gets the age tick
+    A[r] += 1 for every live slot r < *live_dev / rows."""
+    _chk(Opart, Mpart, Lpart, O, U)
+    R, N = Opart.shape[0], Opart.shape[1]
+    if U.numel() != R or not U.is_contiguous() or (A is not None and (A.dtype != torch.int32 or A.numel() != R or
+                                                                      not A.is_cuda)):
+        raise AotbError(f"attn_merge_usage: U must be float32 [{R}] and A int32 [{R}] CUDA tensors")
+    check(lib().aotb_attn_merge_usage_f32(_p(Opart), _p(Mpart), _p(Lpart), _p(O), R, N, H, d_v, O.stride(0), _p(U), _p(A),
+                                          _counter("attn_merge_usage: live_dev", live_dev) if A is not None else None,
+                                          int(rows), int(layers), workspace.data_ptr(), _st(stream)),
+          "aotb_attn_merge_usage_f32")
+    return O
+
+
 def attn_merge_peers(Oparts, Mparts, Lparts, O, splits, H, d_v, stream=None):
     """Merge split-KV partials that live in `len(Oparts)` ranks' buffers (local tensor + peer views of a symmetric-memory
     allocation): Oparts[r] [>=splits, N, H*d_v], Mparts[r] / Lparts[r] [>=splits, H, N]."""
@@ -752,6 +774,18 @@ def ring_advance(live_dev, write_dev, rows, cap_rows, pinned_rows, stream=None):
                                   int(rows), int(cap_rows), int(pinned_rows), _st(stream)), "aotb_ring_advance")
 
 
+def ring_select_usage(live_dev, write_dev, U, A, rows, cap_rows, pinned_rows, stream=None):
+    """Usage policy of the bounded bank, before a store: *write_dev = the next free slot's row while *live_dev < cap_rows,
+    else the row of the unpinned slot with the lowest U / A (A == 0 counts as +inf, ties to the lowest slot); that slot's
+    U (float32 [cap_rows / rows]) and A (int32, same shape) restart at 0."""
+    if U.dtype != torch.float32 or A.dtype != torch.int32 or not U.is_cuda or not A.is_cuda or \
+            U.numel() * rows != cap_rows or A.numel() * rows != cap_rows:
+        raise AotbError(f"ring_select_usage: U must be float32 and A int32 CUDA tensors of {cap_rows} / {rows} slots")
+    check(lib().aotb_ring_select_usage(_counter("ring_select_usage: live_dev", live_dev),
+                                       _counter("ring_select_usage: write_dev", write_dev), U.data_ptr(), A.data_ptr(),
+                                       int(rows), int(cap_rows), int(pinned_rows), _st(stream)), "aotb_ring_select_usage")
+
+
 # ------------------------------------------------------------------ tensor-core long-term attention
 def tc_pack_rows(src, dst, row_off=0, div=1.0, row_off_dev=None, stream=None):
     """src fp32 [rows, H*32] -> dst fp16 [H, cap, 64] rows [row_off, row_off+rows) as [hi(32) | lo(32)]."""
@@ -819,3 +853,27 @@ def gp_attention_tc(Qp, Kp, Vp, N, Tk, O=None, Tk_dev=None, splits=1, exact=True
     if splits > 1 and merge:
         attn_merge(Op, Mp, Lp, O, 1, dv, stream=stream)
     return O
+
+
+def lt_attention_tc_slots(Qp, Kp, Vp, N, Tk_dev, slots, slot_rows, part, exact=True, stream=None):
+    """lt_attention_tc over a bank of `slots` memory slots of `slot_rows` keys (default layout): split z of the partials
+    `part` = (Opart [slots, N, H*32], Mpart [slots, H, N], Lpart [slots, H, N]) is slot z over the live keys *Tk_dev."""
+    H, nq_cap, _ = Qp.shape
+    Op, Mp, Lp = part
+    _chk(Op, Mp, Lp)
+    check(lib().aotb_lt_attn_tc_slots_f16x2(Qp.data_ptr(), nq_cap, Kp.data_ptr(), Vp.data_ptr(), Kp.shape[1], N, 0,
+                                            _counter("lt_attention_tc_slots: Tk_dev", Tk_dev), H, _p(Op), _p(Mp), _p(Lp),
+                                            int(slots), int(slot_rows), (1 if exact else 0) | (4 if LT_SPIN else 0),
+                                            _st(stream)), "aotb_lt_attn_tc_slots_f16x2")
+
+
+def gp_attention_tc_slots(Qp, Kp, Vp, N, Tk_dev, slots, slot_rows, part, exact=True, stream=None):
+    """gp_attention_tc over a bank of `slots` memory slots of `slot_rows` keys: split z of `part` = (Opart [slots, N, dv],
+    Mpart [slots, 1, N], Lpart [slots, 1, N]) is slot z over the live keys *Tk_dev."""
+    Op, Mp, Lp = part
+    _chk(Op, Mp, Lp)
+    check(lib().aotb_gp_attn_tc_slots_f16x2(Qp.data_ptr(), Qp.shape[1], Kp.data_ptr(), Vp.data_ptr(), Kp.shape[1], N, 0,
+                                            _counter("gp_attention_tc_slots: Tk_dev", Tk_dev), Vp.shape[0] * 32, _p(Op),
+                                            _p(Mp), _p(Lp), int(slots), int(slot_rows),
+                                            (1 if exact else 0) | (4 if LT_SPIN else 0), _st(stream)),
+          "aotb_gp_attn_tc_slots_f16x2")

@@ -28,11 +28,12 @@ MAX_AUGS = 8        # aotb_tta_merge_f32 takes up to 8 logit maps
 
 class TTAInferEngine(nn.Module):
     def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1, flip=None, multi_scale=None,
-                 long_term_mem_max=None, precision=None):
+                 long_term_mem_max=None, precision=None, long_term_mem_policy=None):
         """flip / multi_scale default to cfg.TEST_FLIP / cfg.TEST_MULTISCALE; the augmentations are, in this order, every scale
         unflipped and (with flip) flipped, the order of FramePreprocessor's outputs.  long_term_mem_max bounds every
-        augmentation engine's long-term bank and precision ("fp32" | "fp16", default cfg.TEST_PRECISION, else "fp32") is
-        every augmentation engine's (see AOTEngine for both)."""
+        augmentation engine's long-term bank; precision ("fp32" | "fp16", default cfg.TEST_PRECISION, else "fp32") and
+        long_term_mem_policy ("fifo" | "usage", default cfg.TEST_LONG_TERM_MEM_POLICY, else "fifo") are every augmentation
+        engine's (see AOTEngine for all three)."""
         super().__init__()
         cfg = aot_model.cfg
         if getattr(cfg, "MODEL_USE_PREV_PROB", False):
@@ -54,7 +55,7 @@ class TTAInferEngine(nn.Module):
         self.align_corners = cfg.MODEL_ALIGN_CORNERS
         self.aug_engines = [cls(aot_model, gpu_id=gpu_id, long_term_mem_gap=long_term_mem_gap,
                                 short_term_mem_skip=short_term_mem_skip, long_term_mem_max=long_term_mem_max,
-                                precision=precision)
+                                precision=precision, long_term_mem_policy=long_term_mem_policy)
                             for _ in self.flips]
         for e in self.aug_engines:
             e.eval()

@@ -175,6 +175,18 @@ int aotb_attention_f32(const float* Q, int ldq, const float* K, int ldk, const f
                        float* Lout, void* stream);
 int aotb_attn_merge_f32(const float* Opart, const float* Mpart, const float* Lpart, float* O, int R, int N,
                         int H, int d_v, int ldo, void* stream);
+/* The same merge over the R memory slots of a bounded bank (split r = slot r, as aotb_lt_attn_tc_slots_f16x2 and
+ * aotb_gp_attn_tc_slots_f16x2 write them), which also counts how much each slot was read: O is written exactly as
+ * aotb_attn_merge_f32 writes it, and U[r] += sum over (query, head) of the slot's attention mass l_r exp(m_r - m) / L,
+ * scaled by 1 / (layers H N) -- so the `layers` launches of one frame add that frame's mean mass per slot, which sums to 1.
+ * Each CTA sums its masses per slot and the CTA that draws the last ticket adds the CTA sums in CTA order: U is bitwise
+ * reproducible.  A (optional) gets the age tick: A[r] += 1 for every live slot r < *live / rows; pass it in one launch per
+ * frame.  R <= 32.  `workspace` (aotb_attn_merge_usage_workspace_bytes(R) bytes, 16-byte aligned, reusable for any smaller
+ * R) must be zero-filled before its first use: it holds the launch counter, which every launch leaves at zero again. */
+size_t aotb_attn_merge_usage_workspace_bytes(int R);
+int aotb_attn_merge_usage_f32(const float* Opart, const float* Mpart, const float* Lpart, float* O, int R, int N, int H,
+                              int d_v, int ldo, float* U, int* A, const int* live, int rows, int layers, void* workspace,
+                              void* stream);
 
 /* The same merge with every rank's partials read in place over peer memory (sharded long-term bank, BASELINE configs[3]):
  * Oparts / Mparts / Lparts are HOST arrays of `ranks` (<= 8) device pointers -- the local buffer and the NVLink peer mappings
@@ -274,6 +286,14 @@ size_t aotb_lt_attn_tc_smem_bytes(void);
 int aotb_lt_attn_tc_f16x2(const void* Qp, int Nq_cap, const void* Kp, const void* Vp, int kv_cap, int N, int Tk,
                           const int* Tk_dev, int H, float* O, int ldo, float* Opart, float* Mpart, float* Lpart,
                           int splits, int exact, float* dbg, void* stream);
+/* The same attention (default layout) over a bank of memory slots of split_rows keys each: split z covers keys
+ * [z split_rows, (z + 1) split_rows) of the live ones, so with splits slots and the live keys a prefix of whole slots each
+ * partial (Opart [splits][N][H*32], Mpart / Lpart [splits][H][N]) is one slot's; a slot beyond the live keys gets m = -inf,
+ * l = 0.  The live keys must not exceed splits * split_rows.  split_rows need not be a multiple of the 64-key tile.
+ * exact: bit 0 and bit 2 as above; splits >= 2. */
+int aotb_lt_attn_tc_slots_f16x2(const void* Qp, int Nq_cap, const void* Kp, const void* Vp, int kv_cap, int N, int Tk,
+                                const int* Tk_dev, int H, float* Opart, float* Mpart, float* Lpart, int splits, int split_rows,
+                                int exact, void* stream);
 
 /* DeAOT long-term attention as GEMM -> row softmax -> GEMM on the tensor cores (AOTB_DEAOT_LT=gemm):
  * GatedPropagation.forward networks/layers/attention.py:672-704 with 1 head, d_qk = 128, d_v = 1024.  The two GEMMs are
@@ -300,6 +320,10 @@ int aotb_row_softmax_f32(float* S, int ld, int N, int cols, int Tk, const int* T
 int aotb_gp_attn_tc_f16x2(const void* Qp, int Nq_cap, const void* Kp, const void* Vp, int kv_cap, int N, int Tk,
                           const int* Tk_dev, int dv, float* O, int ldo, float* Opart, float* Mpart, float* Lpart,
                           int splits, int exact, void* stream);
+/* Its memory-slot form, as aotb_lt_attn_tc_slots_f16x2: Opart [splits][N][dv], Mpart / Lpart [splits][1][N]. */
+int aotb_gp_attn_tc_slots_f16x2(const void* Qp, int Nq_cap, const void* Kp, const void* Vp, int kv_cap, int N, int Tk,
+                                const int* Tk_dev, int dv, float* Opart, float* Mpart, float* Lpart, int splits, int split_rows,
+                                int exact, void* stream);
 
 /* Long-term memory append in place (replaces torch.cat, networks/engines/aot_engine.py:291-305). */
 int aotb_bank_append_f32(const float* src, int lds, float* bank, int ldb, int rows, int cols, int offset,
@@ -324,6 +348,14 @@ int aotb_bank_ring_store(const float* k_src, int ldk, int k_cols, const float* v
                          float* k_bank, int ldkb, float* v_bank, int ldvb, void* k_packed, void* v_packed, int cap_rows,
                          const int* write, void* stream);
 int aotb_ring_advance(int* live, int* write, int rows, int cap_rows, int pinned_rows, void* stream);
+/* Usage policy of the bounded bank (instead of the FIFO order of aotb_ring_advance's write offset), run before each
+ * aotb_bank_ring_store, with aotb_ring_advance after it for *live: while the bank is not full (*live / rows < cap_rows / rows)
+ * *write = *live, the next free slot; once it is full, *write = s rows for the slot s in [pinned_rows / rows, cap_rows / rows)
+ * with the lowest U[s] / A[s] (A[s] == 0 counts as +inf, ties go to the lowest s).  The chosen slot's U and A are reset to 0.
+ * U / A [cap_rows / rows] are the counters of aotb_attn_merge_usage_f32.  pinned_rows and cap_rows are multiples of rows and
+ * pinned_rows + rows <= cap_rows, so *write always addresses a whole slot of the bank. */
+int aotb_ring_select_usage(const int* live, int* write, float* U, int* A, int rows, int cap_rows, int pinned_rows,
+                           void* stream);
 
 #ifdef __cplusplus
 }
