@@ -14,7 +14,7 @@
 //   warp 4 NWG  TMA producer: the Q tile once, then a ring of K / V stages.
 // The warpgroups run independently (each waits for the stage, each releases it), so one warpgroup's softmax overlaps the
 // other's MMAs.  Layouts of the AOT kernel (all compute the same maxima and, to fp32 rounding, the same P):
-//   tile    NWG = 2, BK = 64                       (default)
+//   tile    NWG = 2, BK = 64                       (default; two co-resident per SM at <= 96 registers)
 //   groups  NWG = 2, BK = 128: half the tile iterations, twice the scores in registers per thread
 //   ahead   NWG = 2, BK = 64, S of tile n + 1 issued before the softmax of tile n, so the tensor cores compute the next
 //           scores while this warpgroup runs ex2 (a second score buffer in registers)
@@ -58,10 +58,16 @@ __device__ __forceinline__ void wgmma_ss(float* d, uint64_t a, uint64_t b, uint3
     else wgmma_ss_n64(d, a, b, scale_d);
 }
 
+// CTAs per SM the register allocation is bounded for.  The tile layout (QC = 1, 64-key tiles, two warpgroups, no second score
+// buffer) fits 96 registers without spilling, so two 9-warp CTAs share an SM and one CTA's MMAs run under the other's
+// softmax; groups, ahead and the DeAOT head shape (QC = 4) spill at that bound and keep one.  pair (5-warp CTAs) takes two.
+template <int QC, int BK, int NWG, bool AHEAD>
+constexpr int attn_tc_min_blocks() { return NWG == 1 || (QC == 1 && BK == 64 && !AHEAD) ? 2 : 1; }
+
 // grid (query tiles of 64 NWG, QC == 1 ? heads : value slices of VC chunks, splits).  Head / slice y reads query and key chunks
 // [y, y + 1) when QC == 1, else [0, QC), and value chunks [y * VC, (y + 1) * VC).
 template <int QC, int VC, int STAGES, bool EXACT, int BK, int NWG, bool AHEAD>
-__global__ void __launch_bounds__(32 * (4 * NWG + 1), NWG == 1 ? 2 : 1)
+__global__ void __launch_bounds__(32 * (4 * NWG + 1), (attn_tc_min_blocks<QC, BK, NWG, AHEAD>()))
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const AttnTcArgs a) {
     using SM = AttnSmem<QC, VC, STAGES, BK, NWG>;
@@ -276,9 +282,9 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     }
 }
 
+// Shared-memory size and carveout of both modes' kernels, set once per process before the first launch or query.
 template <int QC, int VC, int STAGES, int BK, int NWG, bool AHEAD>
-int launch_attn_tc(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnTcArgs& a, dim3 grid,
-                   int exact, cudaStream_t st, const char* what) {
+int configure_attn_tc(const char* what) {
     constexpr int smem = AttnSmem<QC, VC, STAGES, BK, NWG>::TOTAL;
     auto kt = attn_tc_kernel<QC, VC, STAGES, true, BK, NWG, AHEAD>;
     auto kf = attn_tc_kernel<QC, VC, STAGES, false, BK, NWG, AHEAD>;
@@ -286,14 +292,52 @@ int launch_attn_tc(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorM
     if (!configured) {
         cudaError_t e = cudaFuncSetAttribute(kt, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (attn_tc_min_blocks<QC, BK, NWG, AHEAD>() == 2) {
+            // the carveout is a hint: without it the driver may keep enough L1 that only one CTA's shared memory fits
+            if (e == cudaSuccess)
+                e = cudaFuncSetAttribute(kt, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            if (e == cudaSuccess)
+                e = cudaFuncSetAttribute(kf, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        }
         if (e != cudaSuccess) {
             set_error("%s: cudaFuncSetAttribute: %s", what, cudaGetErrorString(e));
             return AOTB_ERR_CUDA;
         }
         configured = true;
     }
-    launch(exact ? kt : kf, grid, dim3(32 * (4 * NWG + 1)), smem, st, tq, tk, tv, a);
+    return AOTB_OK;
+}
+
+template <int QC, int VC, int STAGES, int BK, int NWG, bool AHEAD>
+int launch_attn_tc(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnTcArgs& a, dim3 grid,
+                   int exact, cudaStream_t st, const char* what) {
+    const int rc = configure_attn_tc<QC, VC, STAGES, BK, NWG, AHEAD>(what);
+    if (rc != AOTB_OK) return rc;
+    auto kt = attn_tc_kernel<QC, VC, STAGES, true, BK, NWG, AHEAD>;
+    auto kf = attn_tc_kernel<QC, VC, STAGES, false, BK, NWG, AHEAD>;
+    launch(exact ? kt : kf, grid, dim3(32 * (4 * NWG + 1)), AttnSmem<QC, VC, STAGES, BK, NWG>::TOTAL, st, tq, tk, tv, a);
     return check_launch(what);
+}
+
+// Resident CTAs per SM of one mode's kernel as launch_attn_tc configures it, with its registers per thread and local-memory
+// (spill) bytes per thread.
+template <int QC, int VC, int STAGES, int BK, int NWG, bool AHEAD>
+int attn_tc_occupancy(int exact, int* ctas_per_sm, int* regs, int* local_bytes, const char* what) {
+    const int rc = configure_attn_tc<QC, VC, STAGES, BK, NWG, AHEAD>(what);
+    if (rc != AOTB_OK) return rc;
+    const void* k = exact ? (const void*)attn_tc_kernel<QC, VC, STAGES, true, BK, NWG, AHEAD>
+                          : (const void*)attn_tc_kernel<QC, VC, STAGES, false, BK, NWG, AHEAD>;
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k, 32 * (4 * NWG + 1),
+                                                                  AttnSmem<QC, VC, STAGES, BK, NWG>::TOTAL);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k);
+    if (e != cudaSuccess) {
+        set_error("%s: %s", what, cudaGetErrorString(e));
+        return AOTB_ERR_CUDA;
+    }
+    *regs = fa.numRegs;
+    *local_bytes = (int)fa.localSizeBytes;
+    return AOTB_OK;
 }
 
 }  // namespace tc

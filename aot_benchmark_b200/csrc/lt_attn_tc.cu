@@ -97,6 +97,14 @@ extern "C" int aotb_tc_pack_rows_f16x2(const float* src, int ld, void* dst, int 
 
 extern "C" size_t aotb_lt_attn_tc_smem_bytes(void) { return (size_t)tc::AttnSmem<1, 1, tc::LT_STAGES, 64, 2>::TOTAL; }
 
+// The default ("tile") layout's kernel in one mode (exact bit 0), on the current device: resident CTAs per SM, registers per
+// thread and local-memory bytes per thread.
+extern "C" int aotb_lt_attn_tc_occupancy(int exact, int* ctas_per_sm, int* regs, int* local_bytes) {
+    AOTB_REQUIRE(ctas_per_sm && regs && local_bytes, "aotb_lt_attn_tc_occupancy: bad args");
+    return tc::attn_tc_occupancy<1, 1, tc::LT_STAGES, 64, 2, false>(exact & 1, ctas_per_sm, regs, local_bytes,
+                                                                     "aotb_lt_attn_tc_occupancy");
+}
+
 // Qp [H][Nq_cap][64], Kp/Vp [H][kv_cap][64] packed fp16x2 operands (zero-filled beyond the live rows);
 // O [N][ldo] fp32 (head h at columns h*32).  splits > 1 writes un-normalised partials
 // (Opart [splits][N][H*32], Mpart/Lpart [splits][H][N]) for aotb_attn_merge_f32.

@@ -243,12 +243,21 @@ def fork_join(owner, items, fn):
     return outs
 
 
+# CTAs per SM of the tensor-core attention's "tile" layout: its kernel is register-bounded for two (attn_tc_min_blocks in
+# csrc/attn_tc.cuh) and asks for the shared-memory carveout that holds two; the "groups" / "ahead" layouts keep one.
+# tests/test_gpu_lt_occupancy.py checks that the device keeps this many resident (aotb_lt_attn_tc_occupancy).
+LT_TILE_CTAS_PER_SM = 2
+
+
 def lt_splits(n_queries, heads, tk, sms=132, variant=None):
     """KV-split count for the tensor-core kernel: fill whole waves of CTA slots while keeping >= 2 x 128 keys per split.
-    One CTA = 128 queries x 1 head x 1 split at one CTA per SM ("tile" / "groups" / "ahead" layouts) or 64 queries x 1
-    head x 1 split at two CTAs per SM ("pair" layout)."""
-    pair = (ops.LT_VARIANT if variant is None else variant) == "pair"
-    qrows, slots = (64, 2 * sms) if pair else (128, sms)
+    One CTA = 128 queries x 1 head x 1 split at LT_TILE_CTAS_PER_SM CTAs per SM ("tile" layout) or one ("groups" / "ahead"
+    layouts), or 64 queries x 1 head x 1 split at two CTAs per SM ("pair" layout)."""
+    v = ops.LT_VARIANT if variant is None else variant
+    if v == "pair":
+        qrows, slots = 64, 2 * sms
+    else:
+        qrows, slots = 128, (LT_TILE_CTAS_PER_SM if v == "tile" else 1) * sms
     base = ((n_queries + qrows - 1) // qrows) * heads
     tiles = (tk + 127) // 128
     effs = []

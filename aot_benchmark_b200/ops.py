@@ -810,6 +810,16 @@ LT_VARIANT = os.environ.get("AOTB_LT_VARIANT", "tile")
 LT_SPIN = os.environ.get("AOTB_LT_SPIN", "0") == "1"
 
 
+def lt_attn_tc_occupancy(exact=True):
+    """The default ("tile") layout's kernel in one mode on the current device: (resident CTAs per SM, registers per thread,
+    local-memory bytes per thread)."""
+    import ctypes
+    ctas, regs, local = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    check(lib().aotb_lt_attn_tc_occupancy(1 if exact else 0, ctypes.addressof(ctas), ctypes.addressof(regs),
+                                          ctypes.addressof(local)), "aotb_lt_attn_tc_occupancy")
+    return ctas.value, regs.value, local.value
+
+
 def lt_attention_tc(Qp, Kp, Vp, N, Tk, O=None, Tk_dev=None, splits=1, exact=True, part=None, dbg=None, stream=None,
                     merge=True, variant=None):
     """Qp [H, Nq_cap, 64], Kp/Vp [H, kv_cap, 64] packed fp16x2; O [N, H*32] fp32.

@@ -283,6 +283,10 @@ int aotb_tta_feedback_f32(const float* logits, int h, int w, int NC, int H, int 
 int aotb_tc_pack_rows_f16x2(const float* src, int ld, void* dst, int cap, int rows, int H, int row_off,
                             const int* row_off_dev, float div, void* stream);
 size_t aotb_lt_attn_tc_smem_bytes(void);
+/* The default layout's kernel in one mode (exact bit 0 as below) on the current device, configured as its launches are:
+ * resident CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor), registers per thread and local-memory bytes per
+ * thread (cudaFuncGetAttributes).  The KV-split policy assumes the first is 2 (engine.LT_TILE_CTAS_PER_SM). */
+int aotb_lt_attn_tc_occupancy(int exact, int* ctas_per_sm, int* regs, int* local_bytes);
 int aotb_lt_attn_tc_f16x2(const void* Qp, int Nq_cap, const void* Kp, const void* Vp, int kv_cap, int N, int Tk,
                           const int* Tk_dev, int H, float* O, int ldo, float* Opart, float* Mpart, float* Lpart,
                           int splits, int exact, float* dbg, void* stream);
