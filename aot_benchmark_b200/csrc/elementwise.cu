@@ -33,6 +33,8 @@ __global__ void transpose_kernel(const float* __restrict__ in, float* __restrict
 // image [3][HW] (NCHW, batch 1) -> [HW][4] NHWC with a zero 4th channel (so the stem conv reads 16-byte pixels)
 __global__ void image_to_nhwc4_kernel(const float* __restrict__ in, float4* __restrict__ out, int HW) {
     pdl_sync();
+    in += (size_t)blockIdx.y * 3 * HW;               // image blockIdx.y of a batch [B,3,H,W] -> [B,H,W,4]
+    out += (size_t)blockIdx.y * HW;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x)
         out[i] = make_float4(in[i], in[HW + i], in[2 * HW + i], 0.f);
 }
@@ -244,12 +246,16 @@ extern "C" int aotb_nchw_to_nhwc_f32(const float* in, float* out, int B, int C, 
     return check_launch("aotb_nchw_to_nhwc_f32");
 }
 
-extern "C" int aotb_image_to_nhwc4_f32(const float* in, float* out, int HW, void* stream) {
-    AOTB_REQUIRE(in && out && HW > 0, "aotb_image_to_nhwc4_f32: bad args");
+extern "C" int aotb_image_to_nhwc4_batched_f32(const float* in, float* out, int B, int HW, void* stream) {
+    AOTB_REQUIRE(in && out && B > 0 && B <= 65535 && HW > 0, "aotb_image_to_nhwc4_f32: bad args");
     int g = (HW + 255) / 256;
     if (g > 132 * 8) g = 132 * 8;
-    launch(image_to_nhwc4_kernel, dim3(g), dim3(256), 0, (cudaStream_t)stream, in, reinterpret_cast<float4*>(out), HW);
+    launch(image_to_nhwc4_kernel, dim3(g, B), dim3(256), 0, (cudaStream_t)stream, in, reinterpret_cast<float4*>(out), HW);
     return check_launch("aotb_image_to_nhwc4_f32");
+}
+
+extern "C" int aotb_image_to_nhwc4_f32(const float* in, float* out, int HW, void* stream) {
+    return aotb_image_to_nhwc4_batched_f32(in, out, 1, HW, stream);
 }
 
 extern "C" int aotb_nhwc_to_nchw_f32(const float* in, float* out, int B, int C, int HW, void* stream) {

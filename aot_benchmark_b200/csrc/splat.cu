@@ -10,6 +10,10 @@
 // to its own slot of the workspace (double), and the CTA that takes the last ticket of the launch counter adds the slots in
 // CTA order, runs the two small GEMVs and the final gate (radix softmax or h_sigmoid), and resets the counter: the result
 // does not depend on CTA scheduling, and every launch (or graph replay) starts from a zero counter.
+//
+// Every kernel here also takes a batch of B images stacked densely over pixels (blockIdx.y = image): each image of a batch
+// gets the grid, pixel ranges, workspace partials and counter a one-image launch would give it, so image b of a batched
+// launch is bitwise equal to a one-image launch on image b.
 #include "common.cuh"
 #include <cstdint>
 
@@ -32,6 +36,8 @@ splat_attention_kernel(const float* __restrict__ x, int ldx, int HW, int C, int 
                        const float* __restrict__ b1, int inter, const float* __restrict__ w2, const float* __restrict__ b2,
                        float* __restrict__ att, double* __restrict__ partial, unsigned* __restrict__ counter) {
     pdl_sync();
+    // image blockIdx.y: its pixels here, its CTA partials, its own launch counter and its gate where they are used
+    x += (size_t)blockIdx.y * HW * ldx;
     __shared__ float4 red[SPLAT_THREADS];
     __shared__ float gap[SPLAT_MAX_C];
     __shared__ float hid[SPLAT_MAX_C];
@@ -59,16 +65,16 @@ splat_attention_kernel(const float* __restrict__ x, int ldx, int HW, int C, int 
     for (int c = tid; c < C; c += SPLAT_THREADS) {
         double a = 0.0;
         for (int r = 0; r < R; ++r) a += (double)redf[r * C + c];
-        partial[(size_t)blockIdx.x * C + c] = a;
+        partial[((size_t)blockIdx.y * SPLAT_MAX_CTAS + blockIdx.x) * C + c] = a;
     }
     __threadfence();
     __syncthreads();
-    if (tid == 0) last = atomicAdd(counter, 1u) == gridDim.x - 1 ? 1u : 0u;
+    if (tid == 0) last = atomicAdd(counter + blockIdx.y, 1u) == gridDim.x - 1 ? 1u : 0u;
     __syncthreads();
     if (!last) return;
     __threadfence();
     // ---- last CTA: gap = mean over pixels of the sum of the splits (CTA partials in CTA order)
-    const volatile double* pv = partial;
+    const volatile double* pv = partial + (size_t)blockIdx.y * SPLAT_MAX_CTAS * C;
     for (int c = tid; c < C; c += SPLAT_THREADS) {
         double a = 0.0;
         for (int b = 0; b < (int)gridDim.x; ++b) a += pv[(size_t)b * C + c];
@@ -90,6 +96,8 @@ splat_attention_kernel(const float* __restrict__ x, int ldx, int HW, int C, int 
         logit[k] = a;
     }
     __syncthreads();
+    att += (size_t)blockIdx.y * radix * C;
+    counter += blockIdx.y;
     if (GATE == GATE_HSIGMOID) {
         for (int c = tid; c < C; c += SPLAT_THREADS) att[c] = hsigmoid(logit[c]);
         if (tid == 0) *counter = 0u;
@@ -129,6 +137,9 @@ template <int RADIX>
 __global__ void splat_combine_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ att, float* __restrict__ out,
                                      int ldo, int H, int W, int C, int pool_stride, int Ho, int Wo, int act) {
     pdl_sync();
+    x += (size_t)blockIdx.y * H * W * ldx;              // image blockIdx.y of a batch
+    att += (size_t)blockIdx.y * RADIX * C;
+    out += (size_t)blockIdx.y * Ho * Wo * ldo;
     const int C4 = C >> 2;
     const size_t total = (size_t)Ho * Wo * C4;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -207,34 +218,48 @@ static int grid_for(size_t total) {
 
 using namespace aotb;
 
-extern "C" size_t aotb_splat_workspace_bytes(int C) {
-    return SPLAT_HDR + (size_t)SPLAT_MAX_CTAS * (size_t)(C > 0 ? C : 0) * sizeof(double);
+// B counters in the header, then SPLAT_MAX_CTAS partial rows per image; B = 1 is the one-image layout
+extern "C" size_t aotb_splat_workspace_batched_bytes(int C, int B) {
+    const size_t b = B > 0 ? (size_t)B : 0;
+    const size_t hdr = (b * sizeof(unsigned) + SPLAT_HDR - 1) / SPLAT_HDR * SPLAT_HDR;
+    return (hdr > SPLAT_HDR ? hdr : SPLAT_HDR) + b * (size_t)SPLAT_MAX_CTAS * (size_t)(C > 0 ? C : 0) * sizeof(double);
+}
+
+extern "C" size_t aotb_splat_workspace_bytes(int C) { return aotb_splat_workspace_batched_bytes(C, 1); }
+
+static double* splat_partials(void* workspace, int B) {
+    const size_t hdr = ((size_t)B * sizeof(unsigned) + SPLAT_HDR - 1) / SPLAT_HDR * SPLAT_HDR;
+    return (double*)((uint8_t*)workspace + (hdr > SPLAT_HDR ? hdr : SPLAT_HDR));
+}
+
+extern "C" int aotb_splat_attention_batched_f32(const float* x, int ldx, int B, int HW, int C, int radix, const float* w1,
+                                                const float* b1, int inter, const float* w2, const float* b2, float* att,
+                                                void* workspace, void* stream) {
+    AOTB_REQUIRE(x && w1 && b1 && w2 && b2 && att && workspace, "aotb_splat_attention_f32: null pointer");
+    AOTB_REQUIRE(B > 0 && B <= 65535 && HW > 0 && C > 0 && C % 4 == 0 && C <= SPLAT_MAX_C && inter > 0 &&
+                     inter <= SPLAT_MAX_C && radix >= 2 && radix <= SPLAT_MAX_RADIX && ldx >= radix * C,
+                 "aotb_splat_attention_f32: need B > 0, HW > 0, C %% 4 == 0, C and inter <= %d, 2 <= radix <= %d, "
+                 "ldx >= radix * C", SPLAT_MAX_C, SPLAT_MAX_RADIX);
+    AOTB_REQUIRE(ldx % 4 == 0 && (uintptr_t)x % 16 == 0, "aotb_splat_attention_f32: x needs 16-byte aligned rows");
+    const int rows = (SPLAT_THREADS / (C / 4)) * 8;          // ~8 float4 loads per thread and split
+    int ctas = cdiv(HW, rows);
+    ctas = ctas > SPLAT_MAX_CTAS ? SPLAT_MAX_CTAS : ctas;
+    launch(splat_attention_kernel<GATE_RSOFTMAX>, dim3(ctas, B), dim3(SPLAT_THREADS), 0, (cudaStream_t)stream, x, ldx, HW,
+           C, radix, w1, b1, inter, w2, b2, att, splat_partials(workspace, B), (unsigned*)workspace);
+    return check_launch("aotb_splat_attention_f32");
 }
 
 extern "C" int aotb_splat_attention_f32(const float* x, int ldx, int HW, int C, int radix, const float* w1, const float* b1,
                                         int inter, const float* w2, const float* b2, float* att, void* workspace,
                                         void* stream) {
-    AOTB_REQUIRE(x && w1 && b1 && w2 && b2 && att && workspace, "aotb_splat_attention_f32: null pointer");
-    AOTB_REQUIRE(HW > 0 && C > 0 && C % 4 == 0 && C <= SPLAT_MAX_C && inter > 0 && inter <= SPLAT_MAX_C && radix >= 2 &&
-                     radix <= SPLAT_MAX_RADIX && ldx >= radix * C,
-                 "aotb_splat_attention_f32: need HW > 0, C %% 4 == 0, C and inter <= %d, 2 <= radix <= %d, ldx >= radix * C",
-                 SPLAT_MAX_C, SPLAT_MAX_RADIX);
-    AOTB_REQUIRE(ldx % 4 == 0 && (uintptr_t)x % 16 == 0, "aotb_splat_attention_f32: x needs 16-byte aligned rows");
-    const int rows = (SPLAT_THREADS / (C / 4)) * 8;          // ~8 float4 loads per thread and split
-    int ctas = cdiv(HW, rows);
-    ctas = ctas > SPLAT_MAX_CTAS ? SPLAT_MAX_CTAS : ctas;
-    unsigned* counter = (unsigned*)workspace;
-    double* partial = (double*)((uint8_t*)workspace + SPLAT_HDR);
-    launch(splat_attention_kernel<GATE_RSOFTMAX>, dim3(ctas), dim3(SPLAT_THREADS), 0, (cudaStream_t)stream, x, ldx, HW, C, radix, w1, b1,
-           inter, w2, b2, att, partial, counter);
-    return check_launch("aotb_splat_attention_f32");
+    return aotb_splat_attention_batched_f32(x, ldx, 1, HW, C, radix, w1, b1, inter, w2, b2, att, workspace, stream);
 }
 
-extern "C" int aotb_splat_combine_f32(const float* x, int ldx, const float* att, float* out, int ldo, int H, int W, int C,
-                                      int radix, int pool_stride, void* stream) {
+extern "C" int aotb_splat_combine_batched_f32(const float* x, int ldx, const float* att, float* out, int ldo, int B, int H,
+                                              int W, int C, int radix, int pool_stride, void* stream) {
     AOTB_REQUIRE(x && att && out, "aotb_splat_combine_f32: null pointer");
-    AOTB_REQUIRE(H > 0 && W > 0 && C > 0 && C % 4 == 0 && radix >= 1 && radix <= SPLAT_MAX_RADIX && ldx >= radix * C &&
-                     ldo >= C && pool_stride >= 0,
+    AOTB_REQUIRE(B > 0 && B <= 65535 && H > 0 && W > 0 && C > 0 && C % 4 == 0 && radix >= 1 && radix <= SPLAT_MAX_RADIX &&
+                     ldx >= radix * C && ldo >= C && pool_stride >= 0,
                  "aotb_splat_combine_f32: bad shape");
     AOTB_REQUIRE(ldx % 4 == 0 && ldo % 4 == 0 && (uintptr_t)x % 16 == 0 && (uintptr_t)out % 16 == 0 &&
                      (uintptr_t)att % 16 == 0,
@@ -244,39 +269,55 @@ extern "C" int aotb_splat_combine_f32(const float* x, int ldx, const float* att,
     const size_t total = (size_t)Ho * Wo * (C / 4);
     auto kernel = radix == 1 ? splat_combine_kernel<1> : radix == 2 ? splat_combine_kernel<2>
                 : radix == 3 ? splat_combine_kernel<3> : splat_combine_kernel<4>;
-    launch(kernel, dim3(grid_for(total)), dim3(256), 0, (cudaStream_t)stream, x, ldx, att, out, ldo, H, W, C, pool_stride, Ho,
-           Wo, (int)ACT_NONE);
+    launch(kernel, dim3(grid_for(total), B), dim3(256), 0, (cudaStream_t)stream, x, ldx, att, out, ldo, H, W, C, pool_stride,
+           Ho, Wo, (int)ACT_NONE);
     return check_launch("aotb_splat_combine_f32");
 }
 
-extern "C" int aotb_se_gate_f32(const float* x, int ldx, int HW, int C, const float* w1, const float* b1, int inter,
-                                const float* w2, const float* b2, float* gate, void* workspace, void* stream) {
+extern "C" int aotb_splat_combine_f32(const float* x, int ldx, const float* att, float* out, int ldo, int H, int W, int C,
+                                      int radix, int pool_stride, void* stream) {
+    return aotb_splat_combine_batched_f32(x, ldx, att, out, ldo, 1, H, W, C, radix, pool_stride, stream);
+}
+
+extern "C" int aotb_se_gate_batched_f32(const float* x, int ldx, int B, int HW, int C, const float* w1, const float* b1,
+                                        int inter, const float* w2, const float* b2, float* gate, void* workspace,
+                                        void* stream) {
     AOTB_REQUIRE(x && w1 && b1 && w2 && b2 && gate && workspace, "aotb_se_gate_f32: null pointer");
-    AOTB_REQUIRE(HW > 0 && C > 0 && C % 4 == 0 && C <= SPLAT_MAX_C && inter > 0 && inter <= SPLAT_MAX_C && ldx >= C,
-                 "aotb_se_gate_f32: need HW > 0, C %% 4 == 0, C and inter <= %d, ldx >= C", SPLAT_MAX_C);
+    AOTB_REQUIRE(B > 0 && B <= 65535 && HW > 0 && C > 0 && C % 4 == 0 && C <= SPLAT_MAX_C && inter > 0 &&
+                     inter <= SPLAT_MAX_C && ldx >= C,
+                 "aotb_se_gate_f32: need B > 0, HW > 0, C %% 4 == 0, C and inter <= %d, ldx >= C", SPLAT_MAX_C);
     AOTB_REQUIRE(ldx % 4 == 0 && (uintptr_t)x % 16 == 0, "aotb_se_gate_f32: x needs 16-byte aligned rows");
     const int rows = (SPLAT_THREADS / (C / 4)) * 8;
     int ctas = cdiv(HW, rows);
     ctas = ctas > SPLAT_MAX_CTAS ? SPLAT_MAX_CTAS : ctas;
-    unsigned* counter = (unsigned*)workspace;
-    double* partial = (double*)((uint8_t*)workspace + SPLAT_HDR);
-    launch(splat_attention_kernel<GATE_HSIGMOID>, dim3(ctas), dim3(SPLAT_THREADS), 0, (cudaStream_t)stream, x, ldx, HW, C, 1,
-           w1, b1, inter, w2, b2, gate, partial, counter);
+    launch(splat_attention_kernel<GATE_HSIGMOID>, dim3(ctas, B), dim3(SPLAT_THREADS), 0, (cudaStream_t)stream, x, ldx, HW, C,
+           1, w1, b1, inter, w2, b2, gate, splat_partials(workspace, B), (unsigned*)workspace);
     return check_launch("aotb_se_gate_f32");
 }
 
-extern "C" int aotb_gate_scale_f32(const float* x, int ldx, const float* gate, float* out, int ldo, int HW, int C, int act,
-                                   void* stream) {
+extern "C" int aotb_se_gate_f32(const float* x, int ldx, int HW, int C, const float* w1, const float* b1, int inter,
+                                const float* w2, const float* b2, float* gate, void* workspace, void* stream) {
+    return aotb_se_gate_batched_f32(x, ldx, 1, HW, C, w1, b1, inter, w2, b2, gate, workspace, stream);
+}
+
+extern "C" int aotb_gate_scale_batched_f32(const float* x, int ldx, const float* gate, float* out, int ldo, int B, int HW,
+                                           int C, int act, void* stream) {
     AOTB_REQUIRE(x && gate && out, "aotb_gate_scale_f32: null pointer");
-    AOTB_REQUIRE(HW > 0 && C > 0 && C % 4 == 0 && ldx >= C && ldo >= C && act >= ACT_NONE && act <= ACT_HSWISH,
+    AOTB_REQUIRE(B > 0 && B <= 65535 && HW > 0 && C > 0 && C % 4 == 0 && ldx >= C && ldo >= C && act >= ACT_NONE &&
+                     act <= ACT_HSWISH,
                  "aotb_gate_scale_f32: bad shape or activation");
     AOTB_REQUIRE(ldx % 4 == 0 && ldo % 4 == 0 && (uintptr_t)x % 16 == 0 && (uintptr_t)out % 16 == 0 &&
                      (uintptr_t)gate % 16 == 0,
                  "aotb_gate_scale_f32: 16-byte alignment required");
     const size_t total = (size_t)HW * (C / 4);
-    launch(splat_combine_kernel<1>, dim3(grid_for(total)), dim3(256), 0, (cudaStream_t)stream, x, ldx, gate, out, ldo, 1, HW, C,
-           0, 1, HW, act);
+    launch(splat_combine_kernel<1>, dim3(grid_for(total), B), dim3(256), 0, (cudaStream_t)stream, x, ldx, gate, out, ldo, 1,
+           HW, C, 0, 1, HW, act);
     return check_launch("aotb_gate_scale_f32");
+}
+
+extern "C" int aotb_gate_scale_f32(const float* x, int ldx, const float* gate, float* out, int ldo, int HW, int C, int act,
+                                   void* stream) {
+    return aotb_gate_scale_batched_f32(x, ldx, gate, out, ldo, 1, HW, C, act, stream);
 }
 
 extern "C" int aotb_avgpool_nhwc_f32(const float* in, int ldin, float* out, int ldo, int B, int H, int W, int C, int k,

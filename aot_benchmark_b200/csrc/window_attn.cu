@@ -15,6 +15,9 @@
 //    [(0,0) | (1,0) | (0,1) | (1,1)] with zero padding for odd maps; LayerNorm(4C) and the bias-free reduction reuse
 //    layernorm_kernel and the GEMM.
 //
+// Both kernels take a batch of B token maps stacked densely ([B*H*W] rows, blockIdx.z / blockIdx.y = image): the padding,
+// shift, mask and crop are those of each image, and every image gets the CTAs a one-image launch would give it.
+//
 // Bound: HBM/L2 (each qkv element is read once per use; 2*49*49*32 FMAs per (window, head) is ~1 GFLOP per frame at
 // 592x1040, three orders of magnitude below the encoder's linears).
 #include "common.cuh"
@@ -34,6 +37,8 @@ __global__ void __launch_bounds__(64) window_attn_kernel(const float* __restrict
     __shared__ int sSrc[T];                    // row of the token in the un-padded [H*W] matrix, -1 = padding
     __shared__ int sReg[T];                    // region id of the shifted-window mask (0 when shift == 0)
     pdl_sync();
+    qkv += (size_t)blockIdx.z * H * W * ld;          // image blockIdx.z of a batch
+    out += (size_t)blockIdx.z * H * W * ldo;
     const int tid = threadIdx.x;
     const int head = blockIdx.y;
     const int nwx = Wp / WS;
@@ -144,6 +149,8 @@ __global__ void __launch_bounds__(64) window_attn_kernel(const float* __restrict
 __global__ void patch_merge_kernel(const float* __restrict__ x, int ldx, float* __restrict__ out, int ldo, int H, int W,
                                    int H2, int W2, int C) {
     pdl_sync();
+    x += (size_t)blockIdx.y * H * W * ldx;           // image blockIdx.y of a batch
+    out += (size_t)blockIdx.y * H2 * W2 * ldo;
     const int C4 = C >> 2;
     const size_t total = (size_t)H2 * W2 * 4 * C4;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -163,10 +170,11 @@ __global__ void patch_merge_kernel(const float* __restrict__ x, int ldx, float* 
 
 using namespace aotb;
 
-extern "C" int aotb_window_attention_f32(const float* qkv, int ldqkv, const float* qkv_bias, const float* rel_bias,
-                                         float* out, int ldo, int H, int W, int C, int heads, int window, int shift,
-                                         void* stream) {
-    AOTB_REQUIRE(qkv && qkv_bias && rel_bias && out && H > 0 && W > 0 && heads > 0, "aotb_window_attention_f32: bad args");
+extern "C" int aotb_window_attention_batched_f32(const float* qkv, int ldqkv, const float* qkv_bias, const float* rel_bias,
+                                                 float* out, int ldo, int B, int H, int W, int C, int heads, int window,
+                                                 int shift, void* stream) {
+    AOTB_REQUIRE(qkv && qkv_bias && rel_bias && out && B > 0 && B <= 65535 && H > 0 && W > 0 && heads > 0,
+                 "aotb_window_attention_f32: bad args");
     AOTB_REQUIRE(window == 7 && C == heads * 32,
                  "aotb_window_attention_f32: built for window 7 and head dim 32 (swin_base), got window %d, C/heads %d",
                  window, heads ? C / heads : 0);
@@ -175,20 +183,32 @@ extern "C" int aotb_window_attention_f32(const float* qkv, int ldqkv, const floa
                      ((uintptr_t)qkv_bias % 16 == 0),
                  "aotb_window_attention_f32: 16-byte alignment required");
     const int Hp = cdiv(H, window) * window, Wp = cdiv(W, window) * window;
-    dim3 grid((Hp / window) * (Wp / window), heads);
+    dim3 grid((Hp / window) * (Wp / window), heads, B);
     launch(window_attn_kernel<7, 32>, grid, dim3(64), 0, (cudaStream_t)stream, qkv, ldqkv, qkv_bias, rel_bias, out, ldo, H,
            W, Hp, Wp, C, shift, 0.17677669529663687f);   // head_dim ** -0.5 (:124)
     return check_launch("aotb_window_attention_f32");
 }
 
-extern "C" int aotb_patch_merge_f32(const float* x, int ldx, float* out, int ldo, int H, int W, int C, void* stream) {
-    AOTB_REQUIRE(x && out && H > 0 && W > 0 && C > 0 && C % 4 == 0, "aotb_patch_merge_f32: bad args");
+extern "C" int aotb_window_attention_f32(const float* qkv, int ldqkv, const float* qkv_bias, const float* rel_bias,
+                                         float* out, int ldo, int H, int W, int C, int heads, int window, int shift,
+                                         void* stream) {
+    return aotb_window_attention_batched_f32(qkv, ldqkv, qkv_bias, rel_bias, out, ldo, 1, H, W, C, heads, window, shift,
+                                             stream);
+}
+
+extern "C" int aotb_patch_merge_batched_f32(const float* x, int ldx, float* out, int ldo, int B, int H, int W, int C,
+                                            void* stream) {
+    AOTB_REQUIRE(x && out && B > 0 && B <= 65535 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "aotb_patch_merge_f32: bad args");
     AOTB_REQUIRE(ldx % 4 == 0 && ldo % 4 == 0 && ((uintptr_t)x % 16 == 0) && ((uintptr_t)out % 16 == 0),
                  "aotb_patch_merge_f32: 16-byte alignment required");
     const int H2 = (H + 1) / 2, W2 = (W + 1) / 2;
     const size_t total = (size_t)H2 * W2 * C;
     size_t g = (total + 255) / 256;
     if (g > 132 * 16) g = 132 * 16;
-    launch(patch_merge_kernel, dim3((unsigned)g), dim3(256), 0, (cudaStream_t)stream, x, ldx, out, ldo, H, W, H2, W2, C);
+    launch(patch_merge_kernel, dim3((unsigned)g, B), dim3(256), 0, (cudaStream_t)stream, x, ldx, out, ldo, H, W, H2, W2, C);
     return check_launch("aotb_patch_merge_f32");
+}
+
+extern "C" int aotb_patch_merge_f32(const float* x, int ldx, float* out, int ldo, int H, int W, int C, void* stream) {
+    return aotb_patch_merge_batched_f32(x, ldx, out, ldo, 1, H, W, C, stream);
 }

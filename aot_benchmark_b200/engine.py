@@ -97,6 +97,8 @@ def _apply_pdl():
     lib().aotb_set_pdl(1 if USE_PDL else 0)
     check(lib().aotb_set_conv_tiling(_CONV_TILING_MASK[CONV_TILING]), "aotb_set_conv_tiling")
 BANK_INIT_FRAMES = int(_os.environ.get("AOTB_BANK_FRAMES", "24"))   # initial long-term bank capacity (memory frames)
+# offline_encoder: frames per batched encoder pass (one captured graph per chunk size; DESIGN §8 has the sweep it is chosen from)
+OFFLINE_ENC_CHUNK = 16
 
 
 def _resolve_mem_max(aot_model, long_term_mem_max):
@@ -297,12 +299,18 @@ class EncEmbs(list):
 # image encoder (shared by all sub-engines of an infer engine)
 # =====================================================================================
 class _Encoder:
+    """The image encoder + projection over B frames at once ([B,3,H,W] -> four NHWC [B,h,w,c] maps).  Each batch size has
+    its own activation buffers and its own captured graph (one per plan, H, W and B), so alternating B = 1 frames and
+    B-frame chunks never re-allocates what a graph points at."""
+
     def __init__(self, plan, H, W):
         self.plan = plan
         self.H, self.W = H, W
         dev = plan.device
         self.bufs = {}
         self.dev = dev
+        self.B = 1
+        self._per_b = {1: (self.bufs, None, None)}      # B -> (buffers, GraphCache, graph key)
 
     def _buf(self, key, shape):
         b = self.bufs.get(key)
@@ -311,22 +319,58 @@ class _Encoder:
             self.bufs[key] = b
         return b
 
+    def keep_batch_sizes(self, keep):
+        """Free the activation buffers and captured graph of every batch size not in `keep`; the next call with such a size
+        starts over (eager, then captured)."""
+        self._per_b[self.B] = (self.bufs, getattr(self, "graphs", None), getattr(self, "_gkey", None))
+        drop = [b for b in self._per_b if b not in keep]
+        if any(self._per_b[b][1] is not None and self._per_b[b][1].slots for b in drop):
+            torch.cuda.current_stream().synchronize()      # no replay of a dropped graph is still reading its buffers
+        for b in drop:
+            del self._per_b[b]
+        if self.B not in keep:
+            self.bufs, self.graphs, self._gkey = self._per_b.setdefault(1, ({}, None, None))
+            self.B = 1
+
+    def batch_sizes(self):
+        """The batch sizes whose buffers (and graph) this encoder holds."""
+        return sorted(set(self._per_b) | {self.B})
+
+    def _vec(self, key, n):
+        """A per-image vector of n values: [n] for one frame (the one-image form), [B, n] for a batch."""
+        return self._buf(key, (n,) if self.B == 1 else (self.B, n))
+
+    def _reduce_ws(self, key, C):
+        """Workspace of the deterministic multi-CTA reductions (split attention, squeeze-excite): zero-filled once (launch
+        counters), kept for the encoder's lifetime."""
+        ws = self.bufs.get(key)
+        if ws is None:
+            # the one-frame call keeps its two-argument form (the form every caller of splat_workspace had before batching)
+            ws = self.bufs[key] = ops.splat_workspace(C, self.dev) if self.B == 1 else ops.splat_workspace(C, self.dev, self.B)
+        return ws
+
     @staticmethod
     def _osz(n, k, s, p, d=1):
         return (n + 2 * p - d * (k - 1) - 1) // s + 1
 
     def __call__(self, img, st):
+        """img [B,3,H,W] -> EncEmbs of [B, ...] maps (the encoder's own buffers: the next call with the same B overwrites
+        them)."""
         P = self.plan
-        if img.dim() != 4 or img.shape[0] != 1 or img.shape[1] != 3:
-            raise ValueError("expected an image tensor [1,3,H,W]")
+        if img.dim() != 4 or img.shape[0] < 1 or img.shape[1] != 3:
+            raise ValueError(f"expected an image tensor [B,3,H,W], got {tuple(img.shape)}")
         if P.encoder_name == "swin_base" and (img.shape[2] % 4 or img.shape[3] % 4):
             # PatchEmbed zero-pads right/bottom to a multiple of the 4x4 patch (swin_transformer.py:476-481)
             img = torch.nn.functional.pad(img, (0, -img.shape[3] % 4, 0, -img.shape[2] % 4))
-        H, W = img.shape[2], img.shape[3]
+        B, H, W = img.shape[0], img.shape[2], img.shape[3]
+        if B != self.B:
+            self._per_b[self.B] = (self.bufs, getattr(self, "graphs", None), getattr(self, "_gkey", None))
+            self.bufs, self.graphs, self._gkey = self._per_b.get(B, ({}, None, None))
+            self.B = B
         if getattr(self, "_gkey", None) != (id(P), H, W):
             self.graphs = GraphCache()
             self._gkey = (id(P), H, W)
-        x = self._buf("in", (1, H, W, 4))
+        x = self._buf("in", (B, H, W, 4))
         ops.image_to_nhwc4(img.float(), x, stream=st)        # caller's tensor -> static NHWC4 input (eager)
         nhwc = self.graphs.run("enc", lambda: self._body(x))
         out = EncEmbs(t.permute(0, 3, 1, 2) for t in nhwc)
@@ -347,7 +391,7 @@ class _Encoder:
         else:
             feats = self._mobilenet(x, st)
         f16 = feats[-1]
-        proj = self._buf("proj", (1, f16.shape[1], f16.shape[2], P.C))
+        proj = self._buf("proj", (self.B, f16.shape[1], f16.shape[2], P.C))
         ops.conv2d(f16, P.proj.w, P.proj.b, proj, stream=st)
         return [feats[0], feats[1], feats[2], proj]
 
@@ -355,25 +399,25 @@ class _Encoder:
         e = self.plan.enc
         H, W = x.shape[1], x.shape[2]
         h1, w1 = self._osz(H, 7, 2, 3), self._osz(W, 7, 2, 3)
-        c1 = self._buf("stem", (1, h1, w1, 64))
+        c1 = self._buf("stem", (self.B, h1, w1, 64))
         ops.conv2d(x, e.stem.w, e.stem.b, c1, KH=7, KW=7, stride=2, pad=3, act=A_RELU, stream=st)
         h, w = self._osz(h1, 3, 2, 1), self._osz(w1, 3, 2, 1)
-        cur = self._buf("pool", (1, h, w, 64))
+        cur = self._buf("pool", (self.B, h, w, 64))
         ops.maxpool3x3s2(c1, cur, stream=st)
         feats = []
         for si, blocks in enumerate(e.stages):
             for bi, b in enumerate(blocks):
                 ho, wo = self._osz(h, 3, b.stride, 1), self._osz(w, 3, b.stride, 1)
-                t1 = self._buf(f"s{si}b{bi}t1", (1, h, w, b.c1.cout))
+                t1 = self._buf(f"s{si}b{bi}t1", (self.B, h, w, b.c1.cout))
                 ops.conv2d(cur, b.c1.w, b.c1.b, t1, act=A_RELU, stream=st)
-                t2 = self._buf(f"s{si}b{bi}t2", (1, ho, wo, b.c2.cout))
+                t2 = self._buf(f"s{si}b{bi}t2", (self.B, ho, wo, b.c2.cout))
                 ops.conv2d(t1, b.c2.w, b.c2.b, t2, KH=3, KW=3, stride=b.stride, pad=1, act=A_RELU, stream=st)
                 if b.down is not None:
-                    res = self._buf(f"s{si}ds", (1, ho, wo, b.down.cout))
+                    res = self._buf(f"s{si}ds", (self.B, ho, wo, b.down.cout))
                     ops.conv2d(cur, b.down.w, b.down.b, res, stride=b.stride, stream=st)
                 else:
                     res = cur
-                out = self._buf(f"s{si}o{bi % 2}", (1, ho, wo, b.c3.cout))
+                out = self._buf(f"s{si}o{bi % 2}", (self.B, ho, wo, b.c3.cout))
                 ops.conv2d(t2, b.c3.w, b.c3.b, out, res=res, act=A_RELU, stream=st)
                 cur, h, w = out, ho, wo
             feats.append(cur)
@@ -388,44 +432,42 @@ class _Encoder:
         e = self.plan.enc
         H, W = x.shape[1], x.shape[2]
         h, w = self._osz(H, 3, 2, 1), self._osz(W, 3, 2, 1)
-        s0 = self._buf("stem0", (1, h, w, e.stem[0].cout))
+        s0 = self._buf("stem0", (self.B, h, w, e.stem[0].cout))
         ops.conv2d(x, e.stem[0].w, e.stem[0].b, s0, KH=3, KW=3, stride=2, pad=1, act=A_RELU, stream=st)
-        s1 = self._buf("stem1", (1, h, w, e.stem[1].cout))
+        s1 = self._buf("stem1", (self.B, h, w, e.stem[1].cout))
         ops.conv2d(s0, e.stem[1].w, e.stem[1].b, s1, KH=3, KW=3, pad=1, act=A_RELU, stream=st)
-        s2 = self._buf("stem2", (1, h, w, e.stem[2].cout))
+        s2 = self._buf("stem2", (self.B, h, w, e.stem[2].cout))
         ops.conv2d(s1, e.stem[2].w, e.stem[2].b, s2, KH=3, KW=3, pad=1, act=A_RELU, stream=st)
         h, w = self._osz(h, 3, 2, 1), self._osz(w, 3, 2, 1)
-        cur = self._buf("pool", (1, h, w, s2.shape[3]))
+        cur = self._buf("pool", (self.B, h, w, s2.shape[3]))
         ops.maxpool3x3s2(s2, cur, stream=st)
-        ws = self.bufs.get("splat_ws")         # zero-filled once (launch counter), kept for the encoder's lifetime
-        if ws is None:
-            ws = self.bufs["splat_ws"] = ops.splat_workspace(max(b.gw for blocks in e.stages for b in blocks), self.dev)
+        ws = self._reduce_ws("splat_ws", max(b.gw for blocks in e.stages for b in blocks))
         feats = []
         for si, blocks in enumerate(e.stages):
             for bi, b in enumerate(blocks):
                 gw, s = b.gw, b.stride
                 ho, wo = (ops.pool2d_size(h, 3, s, 1), ops.pool2d_size(w, 3, s, 1)) if s > 1 else (h, w)
-                t1 = self._buf(f"s{si}b{bi}t1", (1, h, w, gw))
+                t1 = self._buf(f"s{si}b{bi}t1", (self.B, h, w, gw))
                 ops.conv2d(cur, b.c1.w, b.c1.b, t1, act=A_RELU, stream=st)
-                t2 = self._buf(f"s{si}b{bi}t2", (1, h, w, 2 * gw))
+                t2 = self._buf(f"s{si}b{bi}t2", (self.B, h, w, 2 * gw))
                 for g, cg in enumerate(b.groups):
                     ops.conv2d(t1[..., g * gw // 2:(g + 1) * gw // 2], cg.w, cg.b, t2[..., g * gw:(g + 1) * gw], KH=3, KW=3,
                                pad=1, act=A_RELU, stream=st)
-                att = self._buf(f"s{si}b{bi}att", (2 * gw,))
+                att = self._vec(f"s{si}b{bi}att", 2 * gw)
                 ops.splat_attention(t2, b.fc1_w, b.fc1_b, b.fc2_w, b.fc2_b, att, ws, stream=st)
-                comb = self._buf(f"s{si}b{bi}sum", (1, ho, wo, gw))
+                comb = self._buf(f"s{si}b{bi}sum", (self.B, ho, wo, gw))
                 ops.splat_combine(t2, att, comb, pool_stride=s if s > 1 else 0, stream=st)
                 if b.down is not None:
                     dsrc = cur
                     if s > 1:                                  # AvgPool2d(s, s, ceil_mode=True, count_include_pad=False)
-                        dsrc = self._buf(f"s{si}dp", (1, ops.pool2d_size(h, s, s, 0, True), ops.pool2d_size(w, s, s, 0, True),
+                        dsrc = self._buf(f"s{si}dp", (self.B, ops.pool2d_size(h, s, s, 0, True), ops.pool2d_size(w, s, s, 0, True),
                                                       cur.shape[3]))
                         ops.avgpool(cur, dsrc, s, s, 0, ceil_mode=True, count_include_pad=False, stream=st)
-                    res = self._buf(f"s{si}ds", (1, ho, wo, b.down.cout))
+                    res = self._buf(f"s{si}ds", (self.B, ho, wo, b.down.cout))
                     ops.conv2d(dsrc, b.down.w, b.down.b, res, stream=st)
                 else:
                     res = cur
-                out = self._buf(f"s{si}o{bi % 2}", (1, ho, wo, b.c3.cout))
+                out = self._buf(f"s{si}o{bi % 2}", (self.B, ho, wo, b.c3.cout))
                 ops.conv2d(comb, b.c3.w, b.c3.b, out, res=res, act=A_RELU, stream=st)
                 cur, h, w = out, ho, wo
             feats.append(cur)
@@ -437,14 +479,15 @@ class _Encoder:
         window partition / shift / padding / mask live inside window_attn_kernel, and the per-stage output norms
         write the NHWC feature maps the decoder reads."""
         e = self.plan.enc
+        B = self.B
         H, W, C = x4.shape[1] // 4, x4.shape[2] // 4, e.embed
-        pe = self._buf("pe", (1, H, W, C))
+        pe = self._buf("pe", (B, H, W, C))
         ops.conv2d(x4, e.patch.w, e.patch.b, pe, KH=4, KW=4, stride=4, pad=0, stream=st)          # PatchEmbed :473-489
-        x = self._buf("s0x", (H * W, C))
-        ops.layernorm(pe.view(H * W, C), e.patch_norm[0], e.patch_norm[1], x, stream=st)
+        x = self._buf("s0x", (B * H * W, C))
+        ops.layernorm(pe.view(B * H * W, C), e.patch_norm[0], e.patch_norm[1], x, stream=st)
         feats = []
         for si, stg in enumerate(e.stages):
-            N = H * W
+            N = B * H * W                               # the B token maps stacked
             ln = self._buf(f"s{si}ln", (N, C))
             qkv = self._buf(f"s{si}qkv", (N, 3 * C))
             att = self._buf(f"s{si}att", (N, C))
@@ -452,21 +495,28 @@ class _Encoder:
             for b in stg.blocks:                                                            # SwinTransformerBlock :257-323
                 ops.layernorm(x, b.norm1[0], b.norm1[1], ln, stream=st)
                 ops.linear(ln, b.qkv_w, b.qkv_b, qkv, stream=st)
-                ops.window_attention(qkv, b.qkv_b, b.relb, att, H, W, stg.heads, b.shift, window=e.window, stream=st)
+                if B == 1:        # the one-frame path issues the one-image call exactly as before batching
+                    ops.window_attention(qkv, b.qkv_b, b.relb, att, H, W, stg.heads, b.shift, window=e.window, stream=st)
+                else:
+                    ops.window_attention(qkv, b.qkv_b, b.relb, att, H, W, stg.heads, b.shift, window=e.window, stream=st,
+                                         B=B)
                 ops.linear(att, b.proj_w, b.proj_b, x, res=x, stream=st)                    # x = shortcut + proj(attn)
                 ops.layernorm(x, b.norm2[0], b.norm2[1], ln, stream=st)
                 ops.linear(ln, b.fc1_w, b.fc1_b, hid, act=A_GELU, stream=st)
                 ops.linear(hid, b.fc2_w, b.fc2_b, x, res=x, stream=st)                      # x = x + mlp(norm2(x))
-            f = self._buf(f"s{si}f", (1, H, W, C))
+            f = self._buf(f"s{si}f", (self.B, H, W, C))
             ops.layernorm(x, stg.norm[0], stg.norm[1], f.view(N, C), stream=st)             # norm{i} on the stage output
             feats.append(f)
             if stg.down is not None:                                                        # PatchMerging :339-365
                 H2, W2 = (H + 1) // 2, (W + 1) // 2
-                mg = self._buf(f"s{si}mg", (H2 * W2, 4 * C))
-                ops.patch_merge(x, mg, H, W, stream=st)
-                mln = self._buf(f"s{si}mln", (H2 * W2, 4 * C))
+                mg = self._buf(f"s{si}mg", (B * H2 * W2, 4 * C))
+                if B == 1:
+                    ops.patch_merge(x, mg, H, W, stream=st)
+                else:
+                    ops.patch_merge(x, mg, H, W, stream=st, B=B)
+                mln = self._buf(f"s{si}mln", (B * H2 * W2, 4 * C))
                 ops.layernorm(mg, stg.down.norm[0], stg.down.norm[1], mln, stream=st)
-                x = self._buf(f"s{si + 1}x", (H2 * W2, 2 * C))
+                x = self._buf(f"s{si + 1}x", (B * H2 * W2, 2 * C))
                 ops.linear(mln, stg.down.w, stg.down.b, x, stream=st)
                 H, W, C = H2, W2, 2 * C
         return feats
@@ -480,36 +530,34 @@ class _Encoder:
         e = self.plan.enc
         H, W = x.shape[1], x.shape[2]
         h, w = self._osz(H, 3, 2, 1), self._osz(W, 3, 2, 1)
-        cur = self._buf("stem", (1, h, w, e.stem.cout))
+        cur = self._buf("stem", (self.B, h, w, e.stem.cout))
         ops.conv2d(x, e.stem.w, e.stem.b, cur, KH=3, KW=3, stride=2, pad=1, act=A_HSWISH, stream=st)
-        ws = self.bufs.get("se_ws")            # zero-filled once (launch counter), kept for the encoder's lifetime
-        if ws is None:
-            ws = self.bufs["se_ws"] = ops.splat_workspace(max(b.dw.cout for b in e.blocks if b.se is not None), self.dev)
+        ws = self._reduce_ws("se_ws", max(b.dw.cout for b in e.blocks if b.se is not None))
         feats = []
         for i, b in enumerate(e.blocks):
             act = A_HSWISH if b.hs else A_RELU
             y = cur
             if b.expand is not None:
-                t = self._buf(f"b{i}e", (1, h, w, b.expand.cout))
+                t = self._buf(f"b{i}e", (self.B, h, w, b.expand.cout))
                 ops.conv2d(y, b.expand.w, b.expand.b, t, act=act, stream=st)
                 y = t
             pad = (b.k - 1) // 2 * b.dil                                       # mobilenetv3.py:119-125
             ho, wo = self._osz(h, b.k, b.stride, pad, b.dil), self._osz(w, b.k, b.stride, pad, b.dil)
-            t = self._buf(f"b{i}d", (1, ho, wo, b.dw.cout))
+            t = self._buf(f"b{i}d", (self.B, ho, wo, b.dw.cout))
             ops.dwconv(y, b.dw.w, b.dw.b, t, K=b.k, stride=b.stride, pad=pad, dil=b.dil,
                        act=A_NONE if b.se is not None else act, stream=st)
             if b.se is not None:
-                gate = self._buf(f"b{i}gate", (b.dw.cout,))
+                gate = self._vec(f"b{i}gate", b.dw.cout)
                 ops.se_gate(t, b.se.w1, b.se.b1, b.se.w2, b.se.b2, gate, ws, stream=st)
-                g = self._buf(f"b{i}g", (1, ho, wo, b.dw.cout))
+                g = self._buf(f"b{i}g", (self.B, ho, wo, b.dw.cout))
                 ops.gate_scale(t, gate, g, act=act, stream=st)
                 t = g
-            o = self._buf(f"b{i}o", (1, ho, wo, b.pw.cout))
+            o = self._buf(f"b{i}o", (self.B, ho, wo, b.pw.cout))
             ops.conv2d(t, b.pw.w, b.pw.b, o, res=cur if b.res else None, stream=st)
             cur, h, w = o, ho, wo
             if b.tap:
                 feats.append(cur)
-        last = self._buf("last", (1, h, w, e.last.cout))
+        last = self._buf("last", (self.B, h, w, e.last.cout))
         ops.conv2d(cur, e.last.w, e.last.b, last, act=A_HSWISH, stream=st)
         feats.append(last)
         return feats
@@ -518,25 +566,25 @@ class _Encoder:
         e = self.plan.enc
         H, W = x.shape[1], x.shape[2]
         h, w = self._osz(H, 3, 2, 1), self._osz(W, 3, 2, 1)
-        cur = self._buf("stem", (1, h, w, 32))
+        cur = self._buf("stem", (self.B, h, w, 32))
         ops.conv2d(x, e.stem.w, e.stem.b, cur, KH=3, KW=3, stride=2, pad=1, act=A_RELU6, stream=st)
         feats = []
         for i, b in enumerate(e.blocks):
             y = cur
             if b.expand is not None:
-                t = self._buf(f"b{i}e", (1, h, w, b.expand.cout))
+                t = self._buf(f"b{i}e", (self.B, h, w, b.expand.cout))
                 ops.conv2d(y, b.expand.w, b.expand.b, t, act=A_RELU6, stream=st)
                 y = t
             pad = b.dil  # (3-1)//2*dil, mobilenetv2.py:41-42
             ho, wo = self._osz(h, 3, b.stride, pad, b.dil), self._osz(w, 3, b.stride, pad, b.dil)
-            t = self._buf(f"b{i}d", (1, ho, wo, b.dw.cout))
+            t = self._buf(f"b{i}d", (self.B, ho, wo, b.dw.cout))
             ops.dwconv(y, b.dw.w, b.dw.b, t, K=3, stride=b.stride, pad=pad, dil=b.dil, act=A_RELU6, stream=st)
-            o = self._buf(f"b{i}o", (1, ho, wo, b.pw.cout))
+            o = self._buf(f"b{i}o", (self.B, ho, wo, b.pw.cout))
             ops.conv2d(t, b.pw.w, b.pw.b, o, res=cur if b.res else None, stream=st)
             cur, h, w = o, ho, wo
             if b.tap:
                 feats.append(cur)
-        last = self._buf("last", (1, h, w, e.last.cout))
+        last = self._buf("last", (self.B, h, w, e.last.cout))
         ops.conv2d(cur, e.last.w, e.last.b, last, act=A_RELU6, stream=st)
         feats.append(last)
         return feats
@@ -598,7 +646,8 @@ class AOTEngine(nn.Module):
         self.enc_hw = None
         self.input_size_2d = None
         self.bank_len = 0
-        self.enable_offline_enc = False
+        self._drop_offline_clip()
+        self._alloc_pending = False   # offline_encoder sized the engine for a new video; add_reference_frame allocates
         self.curr_enc_embs = None
         self.curr_id_embs = None
         self.pred_id_logits = None
@@ -608,6 +657,13 @@ class AOTEngine(nn.Module):
             self.tk_dev.zero_()
             self.wr_dev.zero_()
         self._zero_usage()
+
+    def _drop_offline_clip(self):
+        self.enable_offline_enc = False
+        self.offline_enc_embs = None
+        self.offline_masks = None
+        self.offline_frames = -1
+        self.total_offline_frame_num = 0
 
     def _zero_usage(self):
         if getattr(self._ws, "usage_U", None) is not None:
@@ -868,6 +924,90 @@ class AOTEngine(nn.Module):
             raise RuntimeError("aot_benchmark_b200 engines run on CUDA tensors only (there is no CPU path)")
 
     @_in_precision
+    def offline_encoder(self, all_frames, all_masks=None):
+        """aot_engine.py:147-166 at batch size 1: encode every frame of a stored clip all_frames [T,3,H,W] (CUDA) and keep each
+        frame's features (offline_enc_embs[t], EncEmbs views of the clip's storage; the whole clip stays resident, as in the
+        reference).  all_masks [T,1,H,W] label maps, if given, are kept as offline_masks[t].  Until restart_engine(),
+        add_reference_frame / match_propogate_one_frame read the stored features of their frame step and ignore an image
+        they are handed; add_reference_frame(mask=None) uses the stored mask of its step.  The encoder runs over chunks of
+        OFFLINE_ENC_CHUNK frames, each chunk's maps copied straight into the clip's storage.  A clip of at least one chunk
+        runs every pass at B = OFFLINE_ENC_CHUNK, the last one over the clip's last chunk of frames (overlapping the pass
+        before it; only its new frames are stored), so the encoder keeps one batched set of buffers and one graph whatever
+        the clip lengths; a shorter clip runs as one pass of T frames whose buffers are freed when the call returns.
+        The stored frames reach the LSTT and decoder through the engine's own copy buffers (see _offline_embs), so the
+        offline path has its own graph keys, next to those of the per-frame path."""
+        T = self._check_clip(all_frames, all_masks)
+        st = torch.cuda.current_stream().cuda_stream
+        _apply_pdl()
+        self._P = get_plan(self.AOT)
+        if self._enc is None:
+            self._enc = _Encoder(self._plan(), all_frames.shape[2], all_frames.shape[3])
+        self._enc.plan = self._plan()
+        B = min(OFFLINE_ENC_CHUNK, T)
+        starts = list(range(0, T - B + 1, B))
+        if starts[-1] + B < T:
+            starts.append(T - B)                       # the tail: the last B frames, of which only the new ones are stored
+        store, done = None, 0
+        for t0 in starts:
+            maps = self._enc(all_frames[t0:t0 + B], st).nhwc
+            if store is None:
+                store = [torch.empty((T,) + tuple(m.shape[1:]), dtype=torch.float32, device=m.device) for m in maps]
+            for m, dst in zip(maps, store):
+                c = m.shape[3]
+                ops.eltwise(ops.EW_COPY, m[done - t0:].reshape(-1, c), None, dst[done:t0 + B].view(-1, c), stream=st)
+            done = t0 + B
+        self._enc.keep_batch_sizes((1, OFFLINE_ENC_CHUNK))
+        self.enable_offline_enc = True
+        self.offline_frames = T
+        self.total_offline_frame_num = T
+        self.offline_enc_embs = [self._embs_of([m[t:t + 1] for m in store]) for t in range(T)]
+        self.offline_masks = None if all_masks is None else [all_masks[t:t + 1] for t in range(T)]
+        if self.input_size_2d is None:
+            self.update_size(all_frames.shape[2:], tuple(store[-1].shape[1:3]))
+            self._alloc_pending = True
+
+    @staticmethod
+    def _embs_of(nhwc):
+        out = EncEmbs(t.permute(0, 3, 1, 2) for t in nhwc)
+        out.nhwc = list(nhwc)
+        return out
+
+    def _check_clip(self, all_frames, all_masks):
+        if not isinstance(all_frames, torch.Tensor) or all_frames.dim() != 4 or all_frames.shape[0] < 1 \
+                or all_frames.shape[1] != 3:
+            shape = tuple(all_frames.shape) if isinstance(all_frames, torch.Tensor) else type(all_frames).__name__
+            raise ValueError(f"offline_encoder: all_frames must be a [T,3,H,W] tensor with T >= 1, got {shape}")
+        self._check_img(all_frames)
+        T, _, H, W = all_frames.shape
+        if all_masks is not None:
+            if not isinstance(all_masks, torch.Tensor) or tuple(all_masks.shape) != (T, 1, H, W):
+                shape = tuple(all_masks.shape) if isinstance(all_masks, torch.Tensor) else type(all_masks).__name__
+                raise ValueError(f"offline_encoder: all_masks must be [T,1,H,W] = {(T, 1, H, W)} label maps, got {shape}")
+            self._check_img(all_masks)
+        return T
+
+    def _offline_step(self, step):
+        if not 0 <= step < self.total_offline_frame_num:
+            raise IndexError(f"frame step {step} is outside the clip stored by offline_encoder "
+                             f"({self.total_offline_frame_num} frames: steps 0 .. {self.total_offline_frame_num - 1})")
+        return step
+
+    def _offline_embs(self, step, st):
+        """Copy stored frame `step` into the engine's offline feature buffers and return them.  They are static across
+        frames and videos, so the LSTT and decoder graphs keyed on them are captured once; they are not the per-frame
+        encoder's output buffers, so an engine that runs both paths holds one set of those graphs per path."""
+        src = self.offline_enc_embs[self._offline_step(step)].nhwc
+        key = tuple(tuple(t.shape) for t in src)
+        frame = getattr(self, "_offline_frame", None)
+        if frame is None or frame[0] != key:
+            frame = self._offline_frame = (key, self._embs_of([torch.empty(t.shape, dtype=torch.float32, device=t.device)
+                                                               for t in src]))
+        dst = frame[1]
+        for a, b in zip(src, dst.nhwc):
+            ops.eltwise(ops.EW_COPY, a.reshape(-1, a.shape[3]), None, b.view(-1, b.shape[3]), stream=st)
+        return dst
+
+    @_in_precision
     def assign_identity_from_mask(self, mask, st):
         """one_hot_mask + get_id_emb (aot_engine.py:168-179) fused as a gather (K4)."""
         P = self._plan()
@@ -907,7 +1047,12 @@ class AOTEngine(nn.Module):
             self.obj_nums = obj_nums
         if frame_step == -1:
             frame_step = self.frame_step
-        if img_embs is None and img is None:
+        offline = self.enable_offline_enc and img_embs is None
+        if offline:
+            self._offline_step(frame_step)
+            if mask is None and self.offline_masks is not None:
+                mask = self.offline_masks[frame_step]
+        if img_embs is None and img is None and not offline:
             print('No image for reference frame!')
             exit()
         if mask is None:
@@ -916,14 +1061,18 @@ class AOTEngine(nn.Module):
         st = torch.cuda.current_stream().cuda_stream
         _apply_pdl()
         self._P = get_plan(self.AOT)   # picks up load_state_dict / .to() done since the last video
-        if img_embs is None:
+        if offline:
+            img_embs = self._offline_embs(frame_step, st)      # the stored frame; an image handed here is ignored
+        elif img_embs is None:
             self._check_img(img)
             img_embs = self._encode(img, st)
-        if self.input_size_2d is None:
-            f16 = img_embs.nhwc[-1]
-            in_size = img.shape[2:] if img is not None else (f16.shape[1] * 16, f16.shape[2] * 16)
-            self.update_size(in_size, (f16.shape[1], f16.shape[2]))
+        if self.input_size_2d is None or self._alloc_pending:
+            if self.input_size_2d is None:
+                f16 = img_embs.nhwc[-1]
+                in_size = img.shape[2:] if img is not None else (f16.shape[1] * 16, f16.shape[2] * 16)
+                self.update_size(in_size, (f16.shape[1], f16.shape[2]))
             self._alloc()
+            self._alloc_pending = False
         self.curr_enc_embs = img_embs
         if self.pos_emb is None:
             # the table lives in the workspace, i.e. exactly as long as the captured graphs that read it: re-creating it per
@@ -944,9 +1093,14 @@ class AOTEngine(nn.Module):
 
     @_in_precision
     def match_propogate_one_frame(self, img=None, img_embs=None):
+        offline = img_embs is None and self.enable_offline_enc
+        if offline:
+            self._offline_step(self.frame_step + 1)
         self.frame_step += 1
         st = torch.cuda.current_stream().cuda_stream
-        if img_embs is None:
+        if offline:
+            img_embs = self._offline_embs(self.frame_step, st)   # the stored frame; an image handed here is ignored
+        elif img_embs is None:
             self._check_img(img)
             img_embs = self._encode(img, st)
         self.curr_enc_embs = img_embs
@@ -1560,9 +1714,14 @@ class AOTInferEngine(nn.Module):
 
     def restart_engine(self):
         # keep the engines (and their device buffers) across videos; just reset their state
+        for e in self.aot_engines:
+            e._drop_offline_clip()         # a pooled engine does not keep the previous video's stored clip alive
         self._pool = getattr(self, "_pool", []) + list(self.aot_engines)
         self.aot_engines = []
         self.obj_nums = None
+        self.enable_offline_enc = False
+        self.offline_frames = -1
+        self.total_offline_frame_num = 0
 
     # ------------------------------------------------------------------ > max_aot_obj_num objects (SURVEY 8 f.2)
     # ceil(objects / 10) sub-engines share one encoder pass.  Their LSTT / decoder / memory-update work is independent, so
@@ -1609,11 +1768,8 @@ class AOTInferEngine(nn.Module):
                                                     dtype=torch.float32, device=first.device))
         return ops.soft_logit_aggregation([t if t.is_contiguous() else t.contiguous() for t in all_logits], buf[1], per)
 
-    def add_reference_frame(self, img, mask, obj_nums, frame_step=-1):
-        if isinstance(obj_nums, list):
-            obj_nums = obj_nums[0]
-        self.obj_nums = obj_nums
-        want = max(-(-int(obj_nums) // self.max_aot_obj_num), 1)          # ceil(objects / max_aot_obj_num), at least one
+    def _ensure_engines(self, want):
+        """At least `want` sub-engines, from the pool first, each restarted for the new video."""
         while len(self.aot_engines) < want:
             eng = self._pool.pop(0) if self._pool else self._engine_cls(self.AOT, self.gpu_id, self.long_term_mem_gap,
                                                                        self.short_term_mem_skip,
@@ -1627,9 +1783,30 @@ class AOTInferEngine(nn.Module):
             if self._kv_shard is not None:
                 eng.enable_kv_sharding(*self._kv_shard)
             self.aot_engines.append(eng)
-        masks, counts = self.separate_mask(mask, obj_nums)
-        # engine 0 encodes the frame; the others reuse its feature maps (aot_engine.py:596-607)
+
+    def offline_encoder(self, all_frames, all_masks=None):
+        """Encode a stored clip once for every sub-engine (see AOTEngine.offline_encoder): sub-engine 0 holds the features
+        and the stored label maps, the others are handed its features frame by frame (as in the per-frame path), and
+        add_reference_frame(mask=None) separates the stored mask of its step among the sub-engines."""
+        self._ensure_engines(1)
         first = self.aot_engines[0]
+        first.offline_encoder(all_frames, all_masks)
+        self.enable_offline_enc = True
+        self.offline_frames = first.offline_frames
+        self.total_offline_frame_num = first.total_offline_frame_num
+
+    def add_reference_frame(self, img=None, mask=None, obj_nums=None, frame_step=-1):
+        if isinstance(obj_nums, list):
+            obj_nums = obj_nums[0]
+        self.obj_nums = obj_nums
+        want = max(-(-int(obj_nums) // self.max_aot_obj_num), 1)          # ceil(objects / max_aot_obj_num), at least one
+        self._ensure_engines(want)
+        first = self.aot_engines[0]
+        if mask is None and first.enable_offline_enc and first.offline_masks is not None:
+            mask = first.offline_masks[first._offline_step(first.frame_step if frame_step == -1 else frame_step)]
+        masks, counts = self.separate_mask(mask, obj_nums)
+        # engine 0 encodes the frame (or copies out its stored features); the others reuse its feature maps
+        # (aot_engine.py:596-607)
         first.add_reference_frame(img, masks[0], obj_nums=[counts[0]], frame_step=frame_step)
         embs = first.curr_enc_embs
         if len(self.aot_engines) > 1:
@@ -1641,8 +1818,12 @@ class AOTInferEngine(nn.Module):
         first = self.aot_engines[0]
         if len(self.aot_engines) == 1:
             return first.match_propogate_one_frame(img)
-        first._check_img(img)
-        embs = first._encode(img, torch.cuda.current_stream().cuda_stream)       # shared by all sub-engines
+        st = torch.cuda.current_stream().cuda_stream
+        if first.enable_offline_enc:
+            embs = first._offline_embs(first.frame_step + 1, st)               # the stored frame, shared by all sub-engines
+        else:
+            first._check_img(img)
+            embs = first._encode(img, st)       # shared by all sub-engines
         self._run_engines(lambda i, e: e.match_propogate_one_frame(img, img_embs=embs))
 
     def decode_current_logits(self, output_size=None):

@@ -259,9 +259,12 @@ def nchw_to_nhwc(x, out, stream=None):
 
 
 def image_to_nhwc4(img, out, stream=None):
-    """img [1,3,H,W] -> out [1,H,W,4] (4th channel zero)."""
+    """img [B,3,H,W] -> out [B,H,W,4] (4th channel zero)."""
     _chk(img, out)
-    check(lib().aotb_image_to_nhwc4_f32(_p(img.contiguous()), _p(out), img.shape[2] * img.shape[3], _st(stream)),
+    B = img.shape[0]
+    if tuple(out.shape) != (B, img.shape[2], img.shape[3], 4) or not out.is_contiguous():
+        raise AotbError(f"image_to_nhwc4: out must be a contiguous [{B}, H, W, 4] tensor, got {tuple(out.shape)}")
+    check(lib().aotb_image_to_nhwc4_batched_f32(_p(img.contiguous()), _p(out), B, img.shape[2] * img.shape[3], _st(stream)),
           "aotb_image_to_nhwc4_f32")
     return out
 
@@ -317,30 +320,31 @@ def layernorm(x, gamma, beta, out, add=None, out2=None, stream=None):
     return out
 
 
-def window_attention(qkv, qkv_bias, rel_bias, out, H, W, heads, shift, window=7, stream=None):
-    """Swin (S)W-MSA core: qkv [H*W, 3C], qkv_bias [3C], rel_bias [heads, 49, 49], out [H*W, C]."""
+def window_attention(qkv, qkv_bias, rel_bias, out, H, W, heads, shift, window=7, stream=None, B=1):
+    """Swin (S)W-MSA core: qkv [B*H*W, 3C], qkv_bias [3C], rel_bias [heads, 49, 49], out [B*H*W, C] (B token maps stacked,
+    each padded, shifted and cropped on its own)."""
     _chk(qkv, qkv_bias, rel_bias, out)
     C = out.shape[1]
-    if qkv.shape[0] != H * W or qkv.shape[1] != 3 * C or out.shape[0] != H * W:
-        raise AotbError("window_attention: qkv must be [H*W, 3C], out [H*W, C]")
+    if qkv.shape[0] != B * H * W or qkv.shape[1] != 3 * C or out.shape[0] != B * H * W:
+        raise AotbError("window_attention: qkv must be [B*H*W, 3C], out [B*H*W, C]")
     # the kernel reads rel_bias[head][i][j] and qkv_bias[2C + head * head_dim + c] densely
     T = window * window
     if tuple(rel_bias.shape) != (heads, T, T) or not rel_bias.is_contiguous():
         raise AotbError(f"window_attention: rel_bias must be contiguous [{heads}, {T}, {T}], got {tuple(rel_bias.shape)}")
     if qkv_bias.numel() != 3 * C or not qkv_bias.is_contiguous():
         raise AotbError(f"window_attention: qkv_bias must be contiguous with {3 * C} elements, got {qkv_bias.numel()}")
-    check(lib().aotb_window_attention_f32(_p(qkv), qkv.stride(0), _p(qkv_bias), _p(rel_bias), _p(out), out.stride(0),
-                                          H, W, C, heads, window, shift, _st(stream)), "aotb_window_attention_f32")
+    check(lib().aotb_window_attention_batched_f32(_p(qkv), qkv.stride(0), _p(qkv_bias), _p(rel_bias), _p(out), out.stride(0),
+                                                  B, H, W, C, heads, window, shift, _st(stream)), "aotb_window_attention_f32")
     return out
 
 
-def patch_merge(x, out, H, W, stream=None):
-    """x [H*W, C] -> out [ceil(H/2)*ceil(W/2), 4C] (PatchMerging gather)."""
+def patch_merge(x, out, H, W, stream=None, B=1):
+    """x [B*H*W, C] -> out [B*ceil(H/2)*ceil(W/2), 4C] (PatchMerging gather per map)."""
     _chk(x, out)
     C = x.shape[1]
-    if x.shape[0] != H * W or out.shape[0] != ((H + 1) // 2) * ((W + 1) // 2) or out.shape[1] != 4 * C:
+    if x.shape[0] != B * H * W or out.shape[0] != B * ((H + 1) // 2) * ((W + 1) // 2) or out.shape[1] != 4 * C:
         raise AotbError("patch_merge: shape mismatch")
-    check(lib().aotb_patch_merge_f32(_p(x), x.stride(0), _p(out), out.stride(0), H, W, C, _st(stream)),
+    check(lib().aotb_patch_merge_batched_f32(_p(x), x.stride(0), _p(out), out.stride(0), B, H, W, C, _st(stream)),
           "aotb_patch_merge_f32")
     return out
 
@@ -359,63 +363,80 @@ def groupnorm(x, gamma, beta, out, G, act, workspace, stream=None):
     return out
 
 
-def splat_workspace(C, device):
-    n = lib().aotb_splat_workspace_bytes(C)
-    return torch.zeros((n + 7) // 8, dtype=torch.float64, device=device)      # zero: the launch counter lives in it
+def splat_workspace(C, device, B=1):
+    """Workspace of splat_attention / se_gate over C channels and up to B images per launch."""
+    n = lib().aotb_splat_workspace_batched_bytes(C, B)
+    return torch.zeros((n + 7) // 8, dtype=torch.float64, device=device)      # zero: the launch counters live in it
+
+
+def _splat_rows(x):
+    """x [B,H,W,C'] NHWC or [HW, C'] (one image) -> (B, pixels per image, row stride)."""
+    if x.dim() == 4:
+        return x.shape[0], x.shape[1] * x.shape[2], _nhwc_ld(x)
+    return 1, x.shape[0], x.stride(0)
+
+
+def _check_workspace(name, workspace, C, B):
+    need = lib().aotb_splat_workspace_batched_bytes(C, B)
+    if workspace.numel() * workspace.element_size() < need:
+        raise AotbError(f"{name}: workspace of {workspace.numel() * workspace.element_size()} bytes, {B} images of {C} "
+                        f"channels need {need} (splat_workspace(C, device, B))")
 
 
 def splat_attention(x, w1, b1, w2, b2, att, workspace, radix=2, stream=None):
-    """ResNeSt split attention of one image: x [1,H,W,radix*C] NHWC (or [HW, radix*C]), w1 [C, inter], b1 [inter],
-    w2 [inter, radix*C], b2 [radix*C] -> att [radix*C] (radix-major)."""
+    """ResNeSt split attention per image: x [B,H,W,radix*C] NHWC (or [HW, radix*C] for one image), w1 [C, inter],
+    b1 [inter], w2 [inter, radix*C], b2 [radix*C] -> att [B, radix*C] (or [radix*C]; radix-major).  `workspace` comes
+    from splat_workspace(>= C, device, >= B)."""
     _chk(x, w1, b1, w2, b2, att)
-    x2 = x.reshape(-1, x.shape[-1]) if x.dim() == 4 else x
-    HW, ld = x2.shape[0], (_nhwc_ld(x) if x.dim() == 4 else x.stride(0))
+    B, HW, ld = _splat_rows(x)
     C, inter = w1.shape
-    if w2.shape != (inter, radix * C) or b1.numel() != inter or b2.numel() != radix * C or att.numel() != radix * C \
+    if w2.shape != (inter, radix * C) or b1.numel() != inter or b2.numel() != radix * C or att.numel() != B * radix * C \
             or x.shape[-1] < radix * C or not (w1.is_contiguous() and w2.is_contiguous() and att.is_contiguous()):
-        raise AotbError("splat_attention: shapes x [.., >= radix*C], w1 [C, inter], w2 [inter, radix*C], att [radix*C]")
-    check(lib().aotb_splat_attention_f32(_p(x), ld, HW, C, radix, _p(w1), _p(b1), inter, _p(w2), _p(b2), _p(att),
-                                         workspace.data_ptr(), _st(stream)), "aotb_splat_attention_f32")
+        raise AotbError("splat_attention: shapes x [.., >= radix*C], w1 [C, inter], w2 [inter, radix*C], att [B, radix*C]")
+    _check_workspace("splat_attention", workspace, C, B)
+    check(lib().aotb_splat_attention_batched_f32(_p(x), ld, B, HW, C, radix, _p(w1), _p(b1), inter, _p(w2), _p(b2), _p(att),
+                                                 workspace.data_ptr(), _st(stream)), "aotb_splat_attention_f32")
     return att
 
 
 def splat_combine(x, att, out, radix=2, pool_stride=0, stream=None):
-    """x [1,H,W,radix*C], att [radix*C] -> out [1,Ho,Wo,C] = sum_r att_r * x_r, avg-pooled 3x3 / pool_stride / pad 1 if
-    pool_stride > 0."""
+    """x [B,H,W,radix*C], att [B, radix*C] -> out [B,Ho,Wo,C] = sum_r att_r * x_r per image, avg-pooled 3x3 / pool_stride /
+    pad 1 if pool_stride > 0."""
     _chk(x, att, out)
-    _, H, W, _ = x.shape
+    B, H, W, _ = x.shape
     C = out.shape[3]
     Ho, Wo = (pool2d_size(H, 3, pool_stride, 1), pool2d_size(W, 3, pool_stride, 1)) if pool_stride else (H, W)
-    if att.numel() != radix * C or x.shape[3] < radix * C or tuple(out.shape[1:3]) != (Ho, Wo):
+    if att.numel() != B * radix * C or x.shape[3] < radix * C or tuple(out.shape[:3]) != (B, Ho, Wo):
         raise AotbError(f"splat_combine: x {tuple(x.shape)}, att {tuple(att.shape)}, out {tuple(out.shape)}")
-    check(lib().aotb_splat_combine_f32(_p(x), _nhwc_ld(x), _p(att), _p(out), _nhwc_ld(out), H, W, C, radix, int(pool_stride),
-                                       _st(stream)), "aotb_splat_combine_f32")
+    check(lib().aotb_splat_combine_batched_f32(_p(x), _nhwc_ld(x), _p(att), _p(out), _nhwc_ld(out), B, H, W, C, radix,
+                                               int(pool_stride), _st(stream)), "aotb_splat_combine_f32")
     return out
 
 
 def se_gate(x, w1, b1, w2, b2, gate, workspace, stream=None):
-    """Squeeze-excite gate of one image: x [1,H,W,C] NHWC (or [HW, C]), w1 [C, inter], b1 [inter], w2 [inter, C], b2 [C]
-    -> gate [C] = h_sigmoid(ReLU(mean(x) @ w1 + b1) @ w2 + b2).  `workspace` comes from splat_workspace(>= C)."""
+    """Squeeze-excite gate per image: x [B,H,W,C] NHWC (or [HW, C] for one image), w1 [C, inter], b1 [inter], w2 [inter, C],
+    b2 [C] -> gate [B, C] (or [C]) = h_sigmoid(ReLU(mean(x) @ w1 + b1) @ w2 + b2).  `workspace` comes from
+    splat_workspace(>= C, device, >= B)."""
     _chk(x, w1, b1, w2, b2, gate)
-    x2 = x.reshape(-1, x.shape[-1]) if x.dim() == 4 else x
-    HW, ld = x2.shape[0], (_nhwc_ld(x) if x.dim() == 4 else x.stride(0))
+    B, HW, ld = _splat_rows(x)
     C, inter = w1.shape
-    if w2.shape != (inter, C) or b1.numel() != inter or b2.numel() != C or gate.numel() != C or x.shape[-1] != C \
+    if w2.shape != (inter, C) or b1.numel() != inter or b2.numel() != C or gate.numel() != B * C or x.shape[-1] != C \
             or not (w1.is_contiguous() and w2.is_contiguous() and gate.is_contiguous()):
-        raise AotbError("se_gate: shapes x [.., C], w1 [C, inter], w2 [inter, C], gate [C]")
-    check(lib().aotb_se_gate_f32(_p(x), ld, HW, C, _p(w1), _p(b1), inter, _p(w2), _p(b2), _p(gate), workspace.data_ptr(),
-                                 _st(stream)), "aotb_se_gate_f32")
+        raise AotbError("se_gate: shapes x [.., C], w1 [C, inter], w2 [inter, C], gate [B, C]")
+    _check_workspace("se_gate", workspace, C, B)
+    check(lib().aotb_se_gate_batched_f32(_p(x), ld, B, HW, C, _p(w1), _p(b1), inter, _p(w2), _p(b2), _p(gate),
+                                         workspace.data_ptr(), _st(stream)), "aotb_se_gate_f32")
     return gate
 
 
 def gate_scale(x, gate, out, act=ACT_NONE, stream=None):
-    """out [1,H,W,C] = act(gate[c] * x [1,H,W,C]); x / out may be channel slices."""
+    """out [B,H,W,C] = act(gate[b, c] * x [B,H,W,C]); x / out may be channel slices."""
     _chk(x, gate, out)
     B, H, W, C = x.shape
-    if B != 1 or tuple(out.shape) != (1, H, W, C) or gate.numel() != C:
+    if tuple(out.shape) != (B, H, W, C) or gate.numel() != B * C:
         raise AotbError(f"gate_scale: x {tuple(x.shape)}, gate {tuple(gate.shape)}, out {tuple(out.shape)}")
-    check(lib().aotb_gate_scale_f32(_p(x), _nhwc_ld(x), _p(gate), _p(out), _nhwc_ld(out), H * W, C, int(act), _st(stream)),
-          "aotb_gate_scale_f32")
+    check(lib().aotb_gate_scale_batched_f32(_p(x), _nhwc_ld(x), _p(gate), _p(out), _nhwc_ld(out), B, H * W, C, int(act),
+                                            _st(stream)), "aotb_gate_scale_f32")
     return out
 
 

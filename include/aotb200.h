@@ -91,6 +91,8 @@ int aotb_nchw_to_nhwc_f32(const float* in, float* out, int B, int C, int HW, voi
 int aotb_nhwc_to_nchw_f32(const float* in, float* out, int B, int C, int HW, void* stream);
 /* [3][HW] image -> [HW][4] NHWC with a zero 4th channel (16-byte pixels for the stem convolution). */
 int aotb_image_to_nhwc4_f32(const float* in, float* out, int HW, void* stream);
+/* The same for B images stacked densely: [B][3][HW] -> [B][HW][4]; image b equals a one-image launch on image b. */
+int aotb_image_to_nhwc4_batched_f32(const float* in, float* out, int B, int HW, void* stream);
 
 /* nn.MaxPool2d(3, 2, 1): networks/encoders/resnet.py:79,146. */
 int aotb_maxpool3x3s2_nhwc_f32(const float* in, float* out, int B, int H, int W, int C, void* stream);
@@ -125,10 +127,16 @@ int aotb_layernorm_f32(const float* x, int ldx, const float* gamma, const float*
  * + rel_bias + mask) v per head, heads concatenated, before `proj`.  window must be 7, C == heads * 32. */
 int aotb_window_attention_f32(const float* qkv, int ldqkv, const float* qkv_bias, const float* rel_bias, float* out,
                               int ldo, int H, int W, int C, int heads, int window, int shift, void* stream);
+/* The same for B token maps stacked densely: qkv [B*H*W][ldqkv], out [B*H*W][ldo]; padding, shift, mask and crop are
+ * per image, and image b equals a one-image launch on image b bit for bit. */
+int aotb_window_attention_batched_f32(const float* qkv, int ldqkv, const float* qkv_bias, const float* rel_bias, float* out,
+                                      int ldo, int B, int H, int W, int C, int heads, int window, int shift, void* stream);
 
 /* PatchMerging gather (swin_transformer.py:339-360): x [H*W][ldx] (C channels) -> out [ceil(H/2)*ceil(W/2)][ldo] with
  * 4C channels ordered [(0,0) | (1,0) | (0,1) | (1,1)] of each 2x2 block, zeros outside H x W. */
 int aotb_patch_merge_f32(const float* x, int ldx, float* out, int ldo, int H, int W, int C, void* stream);
+/* The same for B maps stacked densely: x [B*H*W][ldx] -> out [B*ceil(H/2)*ceil(W/2)][ldo], zero padding per image. */
+int aotb_patch_merge_batched_f32(const float* x, int ldx, float* out, int ldo, int B, int H, int W, int C, void* stream);
 
 /* nn.GroupNorm(G, C) over [B][P pixels][C] + activation: networks/layers/basic.py:6-12,18,30-32,75-85.  The workspace
  * (aotb_groupnorm_workspace_bytes(B, G) bytes, reusable for any smaller G) must be zero-filled before its first use: it holds
@@ -161,6 +169,20 @@ int aotb_se_gate_f32(const float* x, int ldx, int HW, int C, const float* w1, co
                      const float* b2, float* gate, void* workspace, void* stream);
 /* out [HW][ldo] = act(gate[c] * x[HW][ldx]) over C channels (the SE product, then the block's activation). */
 int aotb_gate_scale_f32(const float* x, int ldx, const float* gate, float* out, int ldo, int HW, int C, int act, void* stream);
+/* Batched forms of the four kernels above: B images stacked densely over pixels (x [B][HW][ldx], out [B][Ho*Wo][ldo]),
+ * att / gate [B][radix*C].  Every image keeps its own CTA partials and launch counter (reduced in CTA order, as in the
+ * one-image launch), so image b equals a one-image launch on image b bit for bit.  The workspace of the two reductions is
+ * aotb_splat_workspace_batched_bytes(C, B) bytes (B = 1: aotb_splat_workspace_bytes(C)), zero-filled before its first use
+ * and left with zero counters by every launch. */
+size_t aotb_splat_workspace_batched_bytes(int C, int B);
+int aotb_splat_attention_batched_f32(const float* x, int ldx, int B, int HW, int C, int radix, const float* w1, const float* b1,
+                                     int inter, const float* w2, const float* b2, float* att, void* workspace, void* stream);
+int aotb_splat_combine_batched_f32(const float* x, int ldx, const float* att, float* out, int ldo, int B, int H, int W, int C,
+                                   int radix, int pool_stride, void* stream);
+int aotb_se_gate_batched_f32(const float* x, int ldx, int B, int HW, int C, const float* w1, const float* b1, int inter,
+                             const float* w2, const float* b2, float* gate, void* workspace, void* stream);
+int aotb_gate_scale_batched_f32(const float* x, int ldx, const float* gate, float* out, int ldo, int B, int HW, int C, int act,
+                                void* stream);
 /* nn.AvgPool2d(k, s, pad, ceil_mode, count_include_pad) in NHWC, in [B][H][W][ldin] -> out [B][Ho][Wo][ldo] with PyTorch's
  * output extent and divisor rules: networks/encoders/resnest/resnet.py:330-342 (avg_down). */
 int aotb_avgpool_nhwc_f32(const float* in, int ldin, float* out, int ldo, int B, int H, int W, int C, int k, int s, int pad,
