@@ -15,6 +15,7 @@
 // Phase 1 puts window taps on lanes (each lane owns <= 8 taps and walks the D channels with
 // 128-bit loads); phase 2 puts channels on lanes so every tap is one coalesced row read.
 #include "common.cuh"
+#include "tc_common.cuh"
 
 namespace aotb {
 
@@ -393,6 +394,272 @@ static int launch_local_tile(const LocalArgs& a, const float* relv_t, cudaStream
 }
 
 
+// Tensor-core kernel for the AOT head shape (d_att = d_v = 32): one CTA per (8 x 16 query tile, head), one warp per query row
+// of 16 (the M = 16 of mma.sync.m16n8k16).  The K and V halos (22 x 32 positions, fp32) are staged once by cp.async; then every
+// warp walks the 15 window rows dy with an online softmax:
+//   R       [16 q] x [32 c] x [16 dx]      dense: unscaled q . relative_emb_k[dy*15 + dx] + bias (dx = 15 is padding)
+//   S band  [16 q] x [32 c] x [32 hx]      (q/T) . k over the halo row ly + dy; tap dx = hx - lx, the rest of the band is unused
+//   the band goes to the warp's scratch at [lx][dx] and comes back in the accumulator layout of R: s = r + dot (r - 1e8 outside
+//   the frame, attention.py:355-357); p = exp(s - m) with the running row max m
+//   P relv  [16 q] x [16 dx] x [32 c]      dense: the probabilities straight from the score accumulators
+//   P V     [16 q] x [32 hx] x [32 c]      band: P scattered back to [lx][hx] through the scratch (zero off the band)
+// Every product is split fp16x2 (hi.hi + lo.hi + hi.lo into fp32, DESIGN 3.1).  The 32-channel contractions assign thread
+// (g, j) the channels 8j .. 8j+7 (two float4) as its k slots; the 32 output channels are n = 4 g + n-tile, so the V and relv
+// operands are float4 reads and every output row is two float4 stores.  Halo rows use 36 floats: both reads are conflict-free.
+constexpr int LTC_TY = 8, LTC_TX = 16, LTC_HH = LTC_TY + 2 * LR, LTC_HW = 32, LTC_LD = 36, LTC_SS = 17;
+constexpr size_t LTC_SMEM = sizeof(float) * (size_t)(2 * LTC_HH * LTC_HW * LTC_LD + LTC_TY * 16 * LTC_SS);
+
+__device__ __forceinline__ void split2(float x, float y, uint32_t& hi, uint32_t& lo) {
+    hi = tc::cvt_h2(x, y);
+    const float2 h = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+    lo = tc::cvt_h2(x - h.x, y - h.y);
+}
+__device__ __forceinline__ void mma16816(float* d, const uint32_t* a, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                 "{%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// d += A.B in split fp16x2: Ah.Bh + Al.Bh + Ah.Bl
+__device__ __forceinline__ void mma_x3(float* d, const uint32_t* ah, const uint32_t* al, const uint32_t* bh, const uint32_t* bl) {
+    mma16816(d, ah, bh[0], bh[1]);
+    mma16816(d, al, bh[0], bh[1]);
+    mma16816(d, ah, bl[0], bl[1]);
+}
+
+__global__ void __launch_bounds__(256, 1) local_attn_mma_kernel(const LocalArgs p, const float* __restrict__ relv_t) {
+    pdl_sync();
+    constexpr int TX = LTC_TX, HW = LTC_HW, LD = LTC_LD, SS = LTC_SS, NPOS = LTC_HH * LTC_HW;
+    extern __shared__ __align__(16) float smem[];
+    float* ks = smem;                     // [22][32][LD]  K halo (zero outside the frame)
+    float* vs = ks + NPOS * LD;           // [22][32][LD]  V halo
+    const int tid = threadIdx.x, ly = tid >> 5, lane = tid & 31, g4 = lane >> 2, j = lane & 3;
+    float* scr = vs + NPOS * LD + ly * 16 * SS;   // [16][SS] this warp's scores / probabilities at [lx][dx]
+    const int tiles_x = (p.w + TX - 1) / TX;
+    const int ty0 = (blockIdx.x / tiles_x) * LTC_TY, tx0 = (blockIdx.x % tiles_x) * TX;
+    const int g = blockIdx.y;
+
+    for (int f = tid; f < NPOS * 8; f += 256) {
+        const int pos = f >> 3, c4 = (f & 7) * 4;
+        const int yy = ty0 - LR + pos / HW, xx = tx0 - LR + pos % HW;
+        const bool in = yy >= 0 && yy < p.h && xx >= 0 && xx < p.w;
+        const size_t off = (size_t)(yy * p.w + xx);
+        cp_async16(ks + pos * LD + c4, in ? p.k + off * p.ldk + g * 32 + c4 : p.k, in ? 16 : 0);
+        cp_async16(vs + pos * LD + c4, in ? p.v + off * p.ldv + g * 32 + c4 : p.v, in ? 16 : 0);
+    }
+
+    // q fragments of rows lx = g4 and g4 + 8: unscaled for R, divided by T before the split for the dot (attention.py:330)
+    uint32_t qh[2][4], ql[2][4], sh[2][4], sl[2][4];
+    {
+        const int y = ty0 + ly;
+        const float T = p.T;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int x = tx0 + g4 + 8 * r;
+            float4 f[2] = {make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)};
+            if (y < p.h && x < p.w) {
+                const float4* src = reinterpret_cast<const float4*>(p.q + (size_t)(y * p.w + x) * p.ldq + g * 32 + 8 * j);
+                f[0] = __ldg(src);
+                f[1] = __ldg(src + 1);
+            }
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk) {
+                split2(f[kk].x, f[kk].y, qh[kk][r], ql[kk][r]);
+                split2(f[kk].z, f[kk].w, qh[kk][r + 2], ql[kk][r + 2]);
+                split2(f[kk].x / T, f[kk].y / T, sh[kk][r], sl[kk][r]);
+                split2(f[kk].z / T, f[kk].w / T, sh[kk][r + 2], sl[kk][r + 2]);
+            }
+        }
+    }
+    cp_async_wait_all();
+    __syncthreads();
+
+    const float* wk = p.relk_w + (size_t)g * LTAPS * 32 + 8 * j;
+    const float* bk = p.relk_b + g * LTAPS;
+    const float* rv = relv_t + (size_t)g * LTAPS * 32 + 4 * g4;
+    // this thread's relative_emb_k rows (taps dx = 8 nt + g4), biases (dx = 8 nt + 2 j + e) and relv_t rows (dx = 2 j + (t & 1) +
+    // 8 (t >> 1)) of one window row; zero at the padding tap dx = 15.  Loaded one window row ahead, so their L2 latency hides
+    // under the MMAs of the current row.
+    struct RowOps { float4 wf[2][2]; float b[2][2]; float4 rf[4]; };
+    auto load_row = [&](int dy, RowOps& r) {
+        const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt) {
+            const int dxb = 8 * nt + g4;
+            const float4* src = reinterpret_cast<const float4*>(wk + (dy * LW + dxb) * 32);
+            r.wf[nt][0] = dxb < LW ? __ldg(src) : z;
+            r.wf[nt][1] = dxb < LW ? __ldg(src + 1) : z;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int dx = 8 * nt + 2 * j + e;
+                r.b[nt][e] = dx < LW ? __ldg(bk + dy * LW + dx) : 0.f;
+            }
+        }
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+            const int dx = 2 * j + (t & 1) + 8 * (t >> 1);
+            r.rf[t] = dx < LW ? __ldg(reinterpret_cast<const float4*>(rv + (dy * LW + dx) * 32)) : z;
+        }
+    };
+    RowOps nxt;
+    load_row(0, nxt);
+    float o[4][4] = {};
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+#pragma unroll 1
+    for (int dy = 0; dy < LW; ++dy) {
+        const RowOps cur = nxt;
+        if (dy + 1 < LW) load_row(dy + 1, nxt);
+        const int hr = ly + dy;
+        const int yy = ty0 - LR + hr;
+        const bool yin = yy >= 0 && yy < p.h;
+        // ---- R: bias + q . relative_emb_k over the taps dx = 8 nt + g4 of this window row
+        float s[2][4];
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                s[nt][e] = cur.b[nt][e];
+                s[nt][e + 2] = cur.b[nt][e];
+            }
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk) {
+                const float4 f = cur.wf[nt][kk];
+                uint32_t bh[2], bl[2];
+                split2(f.x, f.y, bh[0], bl[0]);
+                split2(f.z, f.w, bh[1], bl[1]);
+                mma_x3(s[nt], qh[kk], ql[kk], bh, bl);
+            }
+        }
+        // ---- S band: (q/T) . k[hx] for the 32 halo positions hx = 8 nt + g4 of halo row hr
+        float sb[4][4] = {};
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+            const float4* kp = reinterpret_cast<const float4*>(ks + (hr * HW + 8 * nt + g4) * LD + 8 * j);
+#pragma unroll
+            for (int kk = 0; kk < 2; ++kk) {
+                const float4 f = kp[kk];
+                uint32_t bh[2], bl[2];
+                split2(f.x, f.y, bh[0], bl[0]);
+                split2(f.z, f.w, bh[1], bl[1]);
+                mma_x3(sb[nt], sh[kk], sl[kk], bh, bl);
+            }
+        }
+        // tap dx = hx - lx of row lx: the dot in frame, -1e8 outside
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int lx = g4 + 8 * (i >> 1), hx = 8 * nt + 2 * j + (i & 1), dx = hx - lx;
+                const int xx = tx0 - LR + hx;
+                if (dx >= 0 && dx < LW) scr[lx * SS + dx] = (yin && xx >= 0 && xx < p.w) ? sb[nt][i] : -1e8f;
+            }
+        __syncwarp();
+        float mx[2] = {m[0], m[1]};
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int lx = g4 + 8 * (i >> 1), dx = 8 * nt + 2 * j + (i & 1);
+                s[nt][i] = dx < LW ? s[nt][i] + scr[lx * SS + dx] : -INFINITY;
+                mx[i >> 1] = fmaxf(mx[i >> 1], s[nt][i]);
+            }
+        __syncwarp();
+        // ---- online softmax over the taps seen so far (row max and sum shared by the 4 lanes of a row)
+        float sc[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+            sc[r] = expf(m[r] - mx[r]);
+            m[r] = mx[r];
+            l[r] *= sc[r];
+        }
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) o[nt][i] *= sc[i >> 1];
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                s[nt][i] = expf(s[nt][i] - m[i >> 1]);          // exp(-inf) = 0 for the padding slot dx = 15
+                l[i >> 1] += s[nt][i];
+                scr[(g4 + 8 * (i >> 1)) * SS + 8 * nt + 2 * j + (i & 1)] = s[nt][i];
+            }
+        // ---- P relv: A = P straight from the score accumulators, B = relv_t rows dy*15 + dx, channels 4 g4 .. 4 g4 + 3
+        {
+            uint32_t ah[4], al[4];
+            split2(s[0][0], s[0][1], ah[0], al[0]);
+            split2(s[0][2], s[0][3], ah[1], al[1]);
+            split2(s[1][0], s[1][1], ah[2], al[2]);
+            split2(s[1][2], s[1][3], ah[3], al[3]);
+            const float* f0 = &cur.rf[0].x; const float* f1 = &cur.rf[1].x; const float* f2 = &cur.rf[2].x; const float* f3 = &cur.rf[3].x;
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) {
+                uint32_t bh[2], bl[2];
+                split2(f0[nt], f1[nt], bh[0], bl[0]);
+                split2(f2[nt], f3[nt], bh[1], bl[1]);
+                mma_x3(o[nt], ah, al, bh, bl);
+            }
+        }
+        __syncwarp();
+        // ---- P V over the band: A[lx][hx] = P[lx][hx - lx] (zero off the band), B = V halo row hr
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+            uint32_t ah[4], al[4];
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {
+                const int lx = g4 + 8 * (t & 1), hx = 16 * kk + 2 * j + 8 * (t >> 1);
+                const float p0 = (hx - lx >= 0 && hx - lx < 16) ? scr[lx * SS + hx - lx] : 0.f;
+                const float p1 = (hx + 1 - lx >= 0 && hx + 1 - lx < 16) ? scr[lx * SS + hx + 1 - lx] : 0.f;
+                split2(p0, p1, ah[t], al[t]);
+            }
+            float4 f[4];
+#pragma unroll
+            for (int t = 0; t < 4; ++t)
+                f[t] = *reinterpret_cast<const float4*>(vs + (hr * HW + 16 * kk + 2 * j + (t & 1) + 8 * (t >> 1)) * LD + 4 * g4);
+            const float* f0 = &f[0].x; const float* f1 = &f[1].x; const float* f2 = &f[2].x; const float* f3 = &f[3].x;
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) {
+                uint32_t bh[2], bl[2];
+                split2(f0[nt], f1[nt], bh[0], bl[0]);
+                split2(f2[nt], f3[nt], bh[1], bl[1]);
+                mma_x3(o[nt], ah, al, bh, bl);
+            }
+        }
+        __syncwarp();
+    }
+    // ---- normalise and store: row g4 + 8 r holds channels 8 j + 4 e + nt in o[nt][2 r + e]
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+        l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+        const int y = ty0 + ly, x = tx0 + g4 + 8 * r;
+        if (y < p.h && x < p.w) {
+            const float inv = 1.f / l[r];
+            float4* dst = reinterpret_cast<float4*>(p.out + (size_t)(y * p.w + x) * p.ldo + g * 32 + 8 * j);
+            dst[0] = make_float4(o[0][2 * r] * inv, o[1][2 * r] * inv, o[2][2 * r] * inv, o[3][2 * r] * inv);
+            dst[1] = make_float4(o[0][2 * r + 1] * inv, o[1][2 * r + 1] * inv, o[2][2 * r + 1] * inv, o[3][2 * r + 1] * inv);
+        }
+    }
+}
+
+static int launch_local_tc(const LocalArgs& a, const float* relv_t, cudaStream_t st) {
+    static bool configured = false;
+    if (!configured) {
+        cudaError_t e = cudaFuncSetAttribute(local_attn_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LTC_SMEM);
+        if (e != cudaSuccess) {
+            set_error("aotb_local_attention_tc_f32: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+            return AOTB_ERR_CUDA;
+        }
+        configured = true;
+    }
+    dim3 grid(cdiv(a.h, LTC_TY) * cdiv(a.w, LTC_TX), a.H);
+    launch(local_attn_mma_kernel, grid, dim3(256), LTC_SMEM, st, a, relv_t);
+    return check_launch("aotb_local_attention_tc_f32");
+}
+
+
 // Tiled kernel for the DeAOT head shape (1 head, d_att = 128, d_v = 1024, no relative_emb_v; attention.py:789-861): the same
 // four passes as local_attn_tile_kernel, with the channel dimensions walked in chunks of 32 through the SAME shared-memory
 // halo buffer:
@@ -637,6 +904,22 @@ extern "C" int aotb_local_attention_tile_f32(const float* q, int ldq, const floa
     a.relk_w = relk_w; a.relk_b = relk_b; a.relv = nullptr; a.out = out; a.ldo = ldo;
     a.h = h; a.w = w; a.H = H; a.T = sqrtf(32.f);
     return launch_local_tile(a, relv_t, (cudaStream_t)stream);
+}
+
+// Tensor-core kernel for the AOT head shape: the arguments of aotb_local_attention_tile_f32.
+extern "C" int aotb_local_attention_tc_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                                           const float* relk_w, const float* relk_b, const float* relv_t, float* out,
+                                           int ldo, int h, int w, int H, void* stream) {
+    AOTB_REQUIRE(q && k && v && relk_w && relk_b && relv_t && out && h > 0 && w > 0 && H > 0,
+                 "aotb_local_attention_tc_f32: bad args");
+    AOTB_REQUIRE(ldq % 4 == 0 && ldk % 4 == 0 && ldv % 4 == 0 && ldo % 4 == 0, "aotb_local_attention_tc_f32: ld %% 4");
+    AOTB_REQUIRE(((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)relk_w | (uintptr_t)relv_t | (uintptr_t)out) % 16 == 0,
+                 "aotb_local_attention_tc_f32: q, k, v, relk_w, relv_t and out must be 16-byte aligned");
+    LocalArgs a;
+    a.q = q; a.ldq = ldq; a.k = k; a.ldk = ldk; a.v = v; a.ldv = ldv;
+    a.relk_w = relk_w; a.relk_b = relk_b; a.relv = nullptr; a.out = out; a.ldo = ldo;
+    a.h = h; a.w = w; a.H = H; a.T = sqrtf(32.f);
+    return launch_local_tc(a, relv_t, (cudaStream_t)stream);
 }
 
 // Tiled kernel for the DeAOT head shape (one head, d_att = 128, d_v = 1024, no relative_emb_v): networks/layers/attention.py:789-861.

@@ -39,7 +39,7 @@ LT_PROBE = None
 #   "simt"     fp32 CUDA-core flash kernel                          (attention_simt.cu)
 import os as _os
 LT_IMPL = _os.environ.get("AOTB_LT_IMPL", "tc_exact")
-LOCAL_IMPL = _os.environ.get("AOTB_LOCAL_IMPL", "tile")      # "tile" (halo in smem) | "warp" (generic kernel)
+LOCAL_IMPL = _os.environ.get("AOTB_LOCAL_IMPL", "tc")   # "tc" (tensor cores, AOT heads) | "tile" (halo in smem) | "warp" (generic)
 # DeAOT long-term attention (1 head, d_qk 128, d_v 1024): "tc" = fused wgmma flash kernel (gp_attn_tc.cu, default) |
 # "gemm" = tensor-core GEMM (Q K^T) -> row softmax -> tensor-core GEMM (P V) over split-fp16 operand copies of the bank
 # (deaot_lt.cu) | "simt" = fp32 CUDA-core flash kernel
@@ -1235,9 +1235,10 @@ class AOTEngine(nn.Module):
             else:
                 gK, gV, Tk = self.bank_K[li], self.bank_V[li], self.bank_len
             self._long_term_attention(li, cQ, gK, gV, Tk, ws.core[:, :C], st)
-            if d == 32 and LOCAL_IMPL == "tile":
-                ops.local_attention_tile(cQ, stK[li], stV[li], Lw.relk_w, Lw.relk_b, Lw.relv_t, ws.core[:, C:], h, w, H,
-                                         stream=st)
+            if d == 32 and LOCAL_IMPL in ops.LOCAL_KERNELS:
+                with ops.local_kernel(LOCAL_IMPL):
+                    ops.local_attention_tile(cQ, stK[li], stV[li], Lw.relk_w, Lw.relk_b, Lw.relv_t, ws.core[:, C:], h, w,
+                                             H, stream=st)
             else:
                 ops.local_attention(cQ, stK[li], stV[li], Lw.relk_w, Lw.relk_b, Lw.relv, ws.core[:, C:], h, w, H, d, d,
                                     stream=st)
@@ -1594,7 +1595,7 @@ class DeAOTEngine(AOTEngine):
                 e1.record()
                 probe.append((e0, e1, 2.0 * N * Tk * (d + C4)))      # FLOPs = 2*N*Tk*(d_qk + d_v), SURVEY 8d
             self._gated_tail(ws.core, ws.catU, Lw.lt_dw, ws.dw[:, :C4], h, w, st)
-            if LOCAL_IMPL == "tile" and d == 128 and C4 == 1024:
+            if LOCAL_IMPL != "warp" and d == 128 and C4 == 1024:
                 ops.local_gated_tile(cQ, stK[li], stV[li], Lw.relk_w, Lw.relk_b, ws.core, h, w, stream=st)
             else:
                 ops.local_attention(cQ, stK[li], stV[li], Lw.relk_w, Lw.relk_b, None, ws.core, h, w, 1, d, C4, stream=st)

@@ -531,12 +531,44 @@ def local_gated_tile(q, k, v, relk_w, relk_b, out, h, w, stream=None):
     return out
 
 
+LOCAL_KERNELS = ("tile", "tc")
+# kernel behind local_attention_tile: "tile" = the fp32 CUDA-core tile kernel, "tc" = the tensor-core kernel of
+# local_attention_tc.  Outside `local_kernel` it is the CUDA-core kernel; the engines select theirs around their call, so
+# the AOT short-term attention has one entry point whichever kernel runs.
+_LOCAL_KERNEL = "tile"
+
+
+@contextlib.contextmanager
+def local_kernel(k):
+    """Run the local_attention_tile calls of the enclosed code on kernel `k` ("tile" | "tc")."""
+    global _LOCAL_KERNEL
+    if k not in LOCAL_KERNELS:
+        raise ValueError(f"local kernel must be one of {LOCAL_KERNELS}, got {k!r}")
+    old, _LOCAL_KERNEL = _LOCAL_KERNEL, k
+    try:
+        yield
+    finally:
+        _LOCAL_KERNEL = old
+
+
 def local_attention_tile(q, k, v, relk_w, relk_b, relv_t, out, h, w, H, stream=None):
-    """AOT head shape (d = 32): halo-in-shared-memory kernel; relv_t [H, 225, 32]."""
+    """AOT head shape (d = 32): halo-in-shared-memory kernel; relv_t [H, 225, 32].  Inside local_kernel("tc"), the
+    tensor-core kernel (local_attention_tc)."""
+    if _LOCAL_KERNEL == "tc":
+        return local_attention_tc(q, k, v, relk_w, relk_b, relv_t, out, h, w, H, stream=stream)
     _chk(q, k, v, relk_w, relk_b, relv_t, out)
     check(lib().aotb_local_attention_tile_f32(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(relk_w),
                                               _p(relk_b), _p(relv_t), _p(out), out.stride(0), h, w, H, _st(stream)),
           "aotb_local_attention_tile_f32")
+    return out
+
+
+def local_attention_tc(q, k, v, relk_w, relk_b, relv_t, out, h, w, H, stream=None):
+    """AOT head shape (d = 32) on the tensor cores, split fp16x2; the arguments of local_attention_tile."""
+    _chk(q, k, v, relk_w, relk_b, relv_t, out)
+    check(lib().aotb_local_attention_tc_f32(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(relk_w),
+                                            _p(relk_b), _p(relv_t), _p(out), out.stride(0), h, w, H, _st(stream)),
+          "aotb_local_attention_tc_f32")
     return out
 
 

@@ -231,6 +231,12 @@ int aotb_local_attention_tile_f32(const float* q, int ldq, const float* k, int l
                                   const float* relk_w, const float* relk_b, const float* relv_t, float* out, int ldo,
                                   int h, int w, int H, void* stream);
 
+/* Same computation and arguments as aotb_local_attention_tile_f32 on the tensor cores (mma.sync, split fp16x2 products with
+ * fp32 accumulation and an fp32 softmax), per 8x16 query tile; q, k, v, relk_w, relv_t and out 16-byte aligned, ldo % 4 == 0. */
+int aotb_local_attention_tc_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                                const float* relk_w, const float* relk_b, const float* relv_t, float* out, int ldo,
+                                int h, int w, int H, void* stream);
+
 /* Same computation for the DeAOT head shape (one head, d_att 128, d_v 1024, no relative_emb_v; attention.py:789-861) with the
  * window halos staged in shared memory per 8x6 query tile and the channels walked in chunks of 32. */
 int aotb_local_gated_tile_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
