@@ -5,6 +5,7 @@ Public surface (mirrors the reference's seam, SURVEY 8b):
     build_engine(name, phase, **kw)       networks/engines/__init__.py:5-21
     EngineConfig(exp, model)              configs/default.py:5-9
     TTAInferEngine(aot_model, ...)        networks/managers/evaluator.py:265-446 with TEST_FLIP / TEST_MULTISCALE
+    MultiVideoInferEngine(aot_model, ...) several independent videos propagated in one batched pass per frame
 """
 from .configs import EngineConfig  # noqa: F401
 from .model import build_vos_model  # noqa: F401
@@ -19,4 +20,7 @@ def __getattr__(name):
     if name == "TTAInferEngine":          # imported on first use, like the engines behind build_engine
         from .tta import TTAInferEngine
         return TTAInferEngine
+    if name == "MultiVideoInferEngine":
+        from .multi_video import MultiVideoInferEngine
+        return MultiVideoInferEngine
     raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

@@ -66,10 +66,16 @@ constexpr int attn_tc_min_blocks() { return NWG == 1 || (QC == 1 && BK == 64 && 
 
 // grid (query tiles of 64 NWG, QC == 1 ? heads : value slices of VC chunks, splits).  Head / slice y reads query and key chunks
 // [y, y + 1) when QC == 1, else [0, QC), and value chunks [y * VC, (y + 1) * VC).
+// The body of one CTA.  A launch over n independent problems (attn_tc_batched_kernel) hands CTA (qt, y, z) of problem b:
+// its query rows start at row b q_stride of Q, its keys at row b kv_stride of K / V, its live key count is Tk_dev[b], and its
+// output rows are [b N, (b + 1) N) of O and of the partials (laid out over n N rows).  The one-problem kernel is b = 0, n = 1.
 template <int QC, int VC, int STAGES, bool EXACT, int BK, int NWG, bool AHEAD>
-__global__ void __launch_bounds__(32 * (4 * NWG + 1), (attn_tc_min_blocks<QC, BK, NWG, AHEAD>()))
-attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-               const __grid_constant__ CUtensorMap tmV, const AttnTcArgs a) {
+__device__ __forceinline__ void attn_tc_cta(const CUtensorMap* tmQp, const CUtensorMap* tmKp, const CUtensorMap* tmVp,
+                                            const AttnTcArgs& a, const int qt, const int b, const int q_stride,
+                                            const int kv_stride, const int nprob) {
+    const CUtensorMap& tmQ = *tmQp;
+    const CUtensorMap& tmK = *tmKp;
+    const CUtensorMap& tmV = *tmVp;
     using SM = AttnSmem<QC, VC, STAGES, BK, NWG>;
     constexpr int BM = SM::BM, TMA_WARP = 4 * NWG, SR = BK / 2;     // SR: score registers per thread
     extern __shared__ uint8_t smem_raw[];
@@ -81,7 +87,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     uint64_t* kv_free = kv_full + STAGES;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int qt = blockIdx.x, y = blockIdx.y, z = blockIdx.z;
+    const int y = blockIdx.y, z = blockIdx.z;
     const int qc0 = QC == 1 ? y : 0, vc0 = y * VC;
     pdl_trigger();
     if (tid == 0) {
@@ -92,7 +98,7 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     __syncthreads();
     pdl_wait();       // the packed operands and the live key count were written by earlier kernels
 
-    const int tk = a.Tk_dev ? *a.Tk_dev : a.Tk;
+    const int tk = a.Tk_dev ? a.Tk_dev[b] : a.Tk;
     const int units = (tk + a.split_unit - 1) / a.split_unit;
     const int per = (units + a.splits - 1) / a.splits;
     const int k0 = min(z * per * a.split_unit, tk), k1 = min((z + 1) * per * a.split_unit, tk);
@@ -104,13 +110,13 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
         if (elect_one() && ntiles > 0) {
             tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
             mbar_arrive_expect_tx(q_full, SM::Q_BYTES);
-            for (int c = 0; c < QC; ++c) tma_load_3d(sQ + c * BM * 128, &tmQ, q_full, 0, qt * BM, qc0 + c);
+            for (int c = 0; c < QC; ++c) tma_load_3d(sQ + c * BM * 128, &tmQ, q_full, 0, b * q_stride + qt * BM, qc0 + c);
             for (int n = 0; n < ntiles; ++n) {
                 const int s = n % STAGES;
                 if (n >= STAGES) mbar_wait(&kv_free[s], ((n / STAGES) - 1) & 1);
                 uint8_t* st = sKV + s * SM::STAGE_BYTES;
                 mbar_arrive_expect_tx(&kv_full[s], SM::STAGE_BYTES);
-                const int key0 = k0 + n * BK;
+                const int key0 = b * kv_stride + k0 + n * BK;
                 for (int c = 0; c < QC; ++c) tma_load_3d(st + c * BK * 128, &tmK, &kv_full[s], 0, key0, qc0 + c);
                 for (int v = 0; v < VC; ++v)
                     tma_load_3d(st + SM::K_BYTES + v * BK * 128, &tmV, &kv_full[s], 0, key0, vc0 + v);
@@ -256,8 +262,9 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
     const int cols = gridDim.y * VC * 32;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const int q = qt * BM + row0 + 8 * h;
-        if (q >= a.N) continue;
+        const int ql = qt * BM + row0 + 8 * h;
+        if (ql >= a.N) continue;
+        const int q = b * a.N + ql;
         const float inv = 1.f / l[h];
 #pragma unroll
         for (int v = 0; v < VC; ++v) {
@@ -270,16 +277,37 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
                     r.x *= inv; r.y *= inv;
                     *reinterpret_cast<float2*>(a.O + (size_t)q * a.ldo + col) = r;
                 } else {
-                    *reinterpret_cast<float2*>(a.Opart + ((size_t)z * a.N + q) * cols + col) = r;
+                    *reinterpret_cast<float2*>(a.Opart + ((size_t)z * nprob * a.N + q) * cols + col) = r;
                 }
             }
         }
         if (a.splits > 1 && (lane & 3) == 0 && (QC == 1 || y == 0)) {
-            const size_t idx = ((size_t)z * (QC == 1 ? gridDim.y : 1) + (QC == 1 ? y : 0)) * a.N + q;
+            const size_t idx = ((size_t)z * (QC == 1 ? gridDim.y : 1) + (QC == 1 ? y : 0)) * nprob * a.N + q;
             a.Mpart[idx] = m[h];
             a.Lpart[idx] = l[h];
         }
     }
+}
+
+template <int QC, int VC, int STAGES, bool EXACT, int BK, int NWG, bool AHEAD>
+__global__ void __launch_bounds__(32 * (4 * NWG + 1), (attn_tc_min_blocks<QC, BK, NWG, AHEAD>()))
+attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+               const __grid_constant__ CUtensorMap tmV, const AttnTcArgs a) {
+    attn_tc_cta<QC, VC, STAGES, EXACT, BK, NWG, AHEAD>(&tmQ, &tmK, &tmV, a, blockIdx.x, 0, 0, 0, 1);
+}
+
+// n independent problems in one launch: grid (n x query tiles of one problem, heads / value slices, splits).
+struct AttnTcBatch {
+    int n, qtiles, q_stride, kv_stride;
+};
+
+template <int QC, int VC, int STAGES, bool EXACT, int BK, int NWG, bool AHEAD>
+__global__ void __launch_bounds__(32 * (4 * NWG + 1), (attn_tc_min_blocks<QC, BK, NWG, AHEAD>()))
+attn_tc_batched_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                       const __grid_constant__ CUtensorMap tmV, const AttnTcArgs a, const AttnTcBatch bt) {
+    const int b = blockIdx.x / bt.qtiles;
+    attn_tc_cta<QC, VC, STAGES, EXACT, BK, NWG, AHEAD>(&tmQ, &tmK, &tmV, a, blockIdx.x - b * bt.qtiles, b, bt.q_stride,
+                                                       bt.kv_stride, bt.n);
 }
 
 // Shared-memory size and carveout of both modes' kernels, set once per process before the first launch or query.
@@ -316,6 +344,32 @@ int launch_attn_tc(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorM
     auto kt = attn_tc_kernel<QC, VC, STAGES, true, BK, NWG, AHEAD>;
     auto kf = attn_tc_kernel<QC, VC, STAGES, false, BK, NWG, AHEAD>;
     launch(exact ? kt : kf, grid, dim3(32 * (4 * NWG + 1)), AttnSmem<QC, VC, STAGES, BK, NWG>::TOTAL, st, tq, tk, tv, a);
+    return check_launch(what);
+}
+
+template <int QC, int VC, int STAGES, int BK, int NWG, bool AHEAD>
+int launch_attn_tc_batched(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnTcArgs& a,
+                           const AttnTcBatch& bt, dim3 grid, int exact, cudaStream_t st, const char* what) {
+    constexpr int smem = AttnSmem<QC, VC, STAGES, BK, NWG>::TOTAL;
+    auto kt = attn_tc_batched_kernel<QC, VC, STAGES, true, BK, NWG, AHEAD>;
+    auto kf = attn_tc_batched_kernel<QC, VC, STAGES, false, BK, NWG, AHEAD>;
+    static bool configured = false;
+    if (!configured) {
+        cudaError_t e = cudaFuncSetAttribute(kt, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(kf, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (attn_tc_min_blocks<QC, BK, NWG, AHEAD>() == 2) {
+            if (e == cudaSuccess)
+                e = cudaFuncSetAttribute(kt, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            if (e == cudaSuccess)
+                e = cudaFuncSetAttribute(kf, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        }
+        if (e != cudaSuccess) {
+            set_error("%s: cudaFuncSetAttribute: %s", what, cudaGetErrorString(e));
+            return AOTB_ERR_CUDA;
+        }
+        configured = true;
+    }
+    launch(exact ? kt : kf, grid, dim3(32 * (4 * NWG + 1)), smem, st, tq, tk, tv, a, bt);
     return check_launch(what);
 }
 

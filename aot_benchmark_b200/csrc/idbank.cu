@@ -74,11 +74,11 @@ __global__ void __launch_bounds__(256) id_embed_kernel(const float* __restrict__
 // [a, b) of one id contributes wp[ky][b][id] - wp[ky][a][id]: ~2 table rows per run instead of one per tap
 // (typically ~40 instead of 289 one-KB rows per output pixel).
 template <bool LN>
-__global__ void __launch_bounds__(256) id_embed_runs_kernel(const float* __restrict__ mask, int Hm, int Wm,
-                                                            const float* __restrict__ wp, const float* __restrict__ bias,
-                                                            const float* __restrict__ ln_g, const float* __restrict__ ln_b,
-                                                            float* __restrict__ out, int ldo, int ho, int wo, int C,
-                                                            int NID, int KS, int stride, int pad) {
+__device__ __forceinline__ void id_embed_runs_cta(const float* __restrict__ mask, int Hm, int Wm,
+                                                  const float* __restrict__ wp, const float* __restrict__ bias,
+                                                  const float* __restrict__ ln_g, const float* __restrict__ ln_b,
+                                                  float* __restrict__ out, int ldo, int ho, int wo, int C,
+                                                  int NID, int KS, int stride, int pad) {
     pdl_sync();
     __shared__ int ids[17 * 17];
     __shared__ int run_pos[17 * 18];     // per row: up to KS runs, stored as (start | end<<8 | id<<16)
@@ -142,6 +142,27 @@ __global__ void __launch_bounds__(256) id_embed_runs_kernel(const float* __restr
         const float rstd = rsqrtf(tq / (float)C + 1e-5f);
         out[(size_t)pix * ldo + c] = d * rstd * __ldg(ln_g + c) + __ldg(ln_b + c);
     }
+}
+
+template <bool LN>
+__global__ void __launch_bounds__(256) id_embed_runs_kernel(const float* __restrict__ mask, int Hm, int Wm,
+                                                            const float* __restrict__ wp, const float* __restrict__ bias,
+                                                            const float* __restrict__ ln_g, const float* __restrict__ ln_b,
+                                                            float* __restrict__ out, int ldo, int ho, int wo, int C,
+                                                            int NID, int KS, int stride, int pad) {
+    id_embed_runs_cta<LN>(mask, Hm, Wm, wp, bias, ln_g, ln_b, out, ldo, ho, wo, C, NID, KS, stride, pad);
+}
+
+// n label maps [n][Hm][Wm] in one launch: map b = blockIdx.y writes output rows [b ho wo, (b + 1) ho wo).
+template <bool LN>
+__global__ void __launch_bounds__(256) id_embed_runs_batched_kernel(const float* __restrict__ mask, int Hm, int Wm,
+                                                                    const float* __restrict__ wp, const float* __restrict__ bias,
+                                                                    const float* __restrict__ ln_g, const float* __restrict__ ln_b,
+                                                                    float* __restrict__ out, int ldo, int ho, int wo, int C,
+                                                                    int NID, int KS, int stride, int pad) {
+    const size_t b = blockIdx.y;
+    id_embed_runs_cta<LN>(mask + b * Hm * Wm, Hm, Wm, wp, bias, ln_g, ln_b, out + b * ho * wo * ldo, ldo, ho, wo, C, NID, KS,
+                          stride, pad);
 }
 
 __device__ __forceinline__ void bl_src(int dst, int in_sz, int out_sz, int align, int& i0, int& i1, float& l1) {
@@ -410,12 +431,9 @@ struct RingStoreArgs {
 };
 
 // One thread per (row, 4 channels) of K then V: the source is read once; the packed rows are the bytes of pack_rows64_kernel
-// with div == 1 (hi = fp16(x), lo = fp16(x - hi), [hi(32) | lo(32)] per 32-channel chunk).
-__global__ void __launch_bounds__(256) bank_ring_store_kernel(const RingStoreArgs a, int rows, int cap_rows,
-                                                              const int* __restrict__ write) {
-    pdl_sync();
-    const int off = *write;
-    if (off < 0 || off + rows > cap_rows) return;      // never write outside the bank, whatever the counter holds
+// with div == 1 (hi = fp16(x), lo = fp16(x - hi), [hi(32) | lo(32)] per 32-channel chunk).  Bank
+// rows from `off`; the packed banks' 32-channel chunks are head_rows rows apart.
+__device__ __forceinline__ void ring_store_rows(const RingStoreArgs& a, int rows, int head_rows, int off) {
     const int per_row = a.c4[0] + a.c4[1];
     const size_t total = (size_t)rows * per_row;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -433,7 +451,7 @@ __global__ void __launch_bounds__(256) bank_ring_store_kernel(const RingStoreArg
             const __half2 h0 = __floats2half2_rn(v.x, v.y), h1 = __floats2half2_rn(v.z, v.w);
             const __half2 l0 = __floats2half2_rn(v.x - __low2float(h0), v.y - __high2float(h0));
             const __half2 l1 = __floats2half2_rn(v.z - __low2float(h1), v.w - __high2float(h1));
-            __half* d = packed + ((size_t)(j >> 3) * cap_rows + off + r) * 64 + (j & 7) * 4;
+            __half* d = packed + ((size_t)(j >> 3) * head_rows + off + r) * 64 + (j & 7) * 4;
             uint2 hi, lo;
             hi.x = *reinterpret_cast<const unsigned*>(&h0); hi.y = *reinterpret_cast<const unsigned*>(&h1);
             lo.x = *reinterpret_cast<const unsigned*>(&l0); lo.y = *reinterpret_cast<const unsigned*>(&l1);
@@ -441,6 +459,34 @@ __global__ void __launch_bounds__(256) bank_ring_store_kernel(const RingStoreArg
             *reinterpret_cast<uint2*>(d + 32) = lo;
         }
     }
+}
+
+__global__ void __launch_bounds__(256) bank_ring_store_kernel(const RingStoreArgs a, int rows, int cap_rows,
+                                                              const int* __restrict__ write) {
+    pdl_sync();
+    const int off = *write;
+    if (off < 0 || off + rows > cap_rows) return;      // never write outside the bank, whatever the counter holds
+    ring_store_rows(a, rows, cap_rows, off);
+}
+
+// n banks of cap_rows rows each, stacked (bank b = rows [b cap_rows, (b + 1) cap_rows) of every copy; the packed copies'
+// chunks are head_rows = n_banks cap_rows apart): bank b = blockIdx.y stores source rows [b rows, (b + 1) rows) at its own
+// write offset write[b] when store[b] != 0.
+__global__ void __launch_bounds__(256) bank_ring_store_batched_kernel(const RingStoreArgs a, int rows, int cap_rows,
+                                                                      int head_rows, const int* __restrict__ write,
+                                                                      const int* __restrict__ store) {
+    pdl_sync();
+    const int b = blockIdx.y;
+    if (!store[b]) return;
+    const int off = write[b];
+    if (off < 0 || off + rows > cap_rows) return;
+    RingStoreArgs ab = a;
+    for (int i = 0; i < 2; ++i) {
+        ab.src[i] += (size_t)b * rows * a.ld[i];
+        if (ab.bank[i]) ab.bank[i] += (size_t)b * cap_rows * a.ldb[i];
+        if (ab.packed[i]) ab.packed[i] += (size_t)b * cap_rows * 64;
+    }
+    ring_store_rows(ab, rows, head_rows, off);
 }
 
 // After a store of `rows` rows: one more frame is live until the bank is full; the write offset moves on by one frame and
@@ -451,6 +497,18 @@ __global__ void ring_advance_kernel(int* live, int* write, int rows, int cap_row
     int w = *write + rows;
     if (w + rows > cap_rows) w = pinned_rows;
     *write = w;
+}
+
+// ring_advance_kernel for n banks, bank b only when store[b] != 0.
+__global__ void ring_advance_batched_kernel(int* live, int* write, const int* store, int n, int rows, int cap_rows,
+                                            int pinned_rows) {
+    pdl_sync();
+    const int b = threadIdx.x;
+    if (b >= n || !store[b]) return;
+    live[b] = min(live[b] + rows, cap_rows);
+    int w = write[b] + rows;
+    if (w + rows > cap_rows) w = pinned_rows;
+    write[b] = w;
 }
 
 // Usage policy of the bounded bank, before a store: the next free slot while the bank is not full, else the unpinned slot
@@ -658,4 +716,66 @@ extern "C" int aotb_ring_select_usage(const int* live, int* write, float* U, int
                  "cap_rows (rows %d, cap_rows %d, pinned_rows %d)", rows, cap_rows, pinned_rows);
     launch(ring_select_usage_kernel, dim3(1), dim3(1), 0, (cudaStream_t)stream, live, write, U, A, rows, cap_rows, pinned_rows);
     return check_launch("aotb_ring_select_usage");
+}
+
+extern "C" int aotb_id_embed_runs_batched_f32(const float* mask, int n, int Hm, int Wm, const float* wp, const float* bias,
+                                              const float* ln_gamma, const float* ln_beta, float* out, int ldo, int C, int nid,
+                                              int ksize, int stride, int pad, void* stream) {
+    AOTB_REQUIRE(mask && wp && bias && out && n >= 1 && n <= 65535 && Hm > 0 && Wm > 0,
+                 "aotb_id_embed_runs_batched_f32: bad args");
+    AOTB_REQUIRE(ksize <= 17 && ksize > 0 && stride > 0 && C == 256 && nid < 128,
+                 "aotb_id_embed_runs_batched_f32: unsupported shape");
+    const int ho = (Hm + 2 * pad - ksize) / stride + 1, wo = (Wm + 2 * pad - ksize) / stride + 1;
+    AOTB_REQUIRE(ho > 0 && wo > 0, "aotb_id_embed_runs_batched_f32: empty output");
+    cudaStream_t st = (cudaStream_t)stream;
+    const dim3 grid(ho * wo, n);
+    if (ln_gamma) {
+        AOTB_REQUIRE(ln_beta, "aotb_id_embed_runs_batched_f32: ln_beta");
+        launch(id_embed_runs_batched_kernel<true>, grid, dim3(256), 0, st, mask, Hm, Wm, wp, bias, ln_gamma, ln_beta, out, ldo,
+               ho, wo, C, nid, ksize, stride, pad);
+    } else {
+        launch(id_embed_runs_batched_kernel<false>, grid, dim3(256), 0, st, mask, Hm, Wm, wp, bias, nullptr, nullptr, out, ldo,
+               ho, wo, C, nid, ksize, stride, pad);
+    }
+    return check_launch("aotb_id_embed_runs_batched_f32");
+}
+
+extern "C" int aotb_bank_ring_store_batched(const float* k_src, int ldk, int k_cols, const float* v_src, int ldv, int v_cols,
+                                            int rows, int n, float* k_bank, int ldkb, float* v_bank, int ldvb, void* k_packed,
+                                            void* v_packed, int cap_rows, int head_rows, const int* write, const int* store,
+                                            void* stream) {
+    AOTB_REQUIRE(k_src && v_src && write && store && rows > 0 && rows <= cap_rows && n >= 1 && n <= 65535,
+                 "aotb_bank_ring_store_batched: bad args");
+    AOTB_REQUIRE(k_bank || v_bank || k_packed || v_packed, "aotb_bank_ring_store_batched: no destination");
+    AOTB_REQUIRE((long long)n * cap_rows <= head_rows, "aotb_bank_ring_store_batched: packed chunk stride");
+    AOTB_REQUIRE(k_cols > 0 && v_cols > 0 && k_cols % 4 == 0 && v_cols % 4 == 0 && ldk % 4 == 0 && ldv % 4 == 0 &&
+                 ldk >= k_cols && ldv >= v_cols, "aotb_bank_ring_store_batched: columns and row strides must be multiples of 4");
+    AOTB_REQUIRE((!k_bank || (ldkb % 4 == 0 && ldkb >= k_cols)) && (!v_bank || (ldvb % 4 == 0 && ldvb >= v_cols)),
+                 "aotb_bank_ring_store_batched: bank row stride");
+    AOTB_REQUIRE((!k_packed || k_cols % 32 == 0) && (!v_packed || v_cols % 32 == 0),
+                 "aotb_bank_ring_store_batched: a packed copy needs a multiple of 32 channels");
+    AOTB_REQUIRE(((uintptr_t)k_src | (uintptr_t)v_src | (uintptr_t)k_bank | (uintptr_t)v_bank | (uintptr_t)k_packed |
+                  (uintptr_t)v_packed) % 16 == 0, "aotb_bank_ring_store_batched: alignment");
+    RingStoreArgs a;
+    a.src[0] = k_src; a.src[1] = v_src; a.bank[0] = k_bank; a.bank[1] = v_bank;
+    a.packed[0] = (__half*)k_packed; a.packed[1] = (__half*)v_packed;
+    a.ld[0] = ldk; a.ld[1] = ldv; a.ldb[0] = ldkb; a.ldb[1] = ldvb; a.c4[0] = k_cols / 4; a.c4[1] = v_cols / 4;
+    const size_t total = (size_t)rows * (a.c4[0] + a.c4[1]);
+    int g = (int)((total + 255) / 256);
+    if (g > 132 * 8) g = 132 * 8;
+    launch(bank_ring_store_batched_kernel, dim3(g, n), dim3(256), 0, (cudaStream_t)stream, a, rows, cap_rows, head_rows, write,
+           store);
+    return check_launch("aotb_bank_ring_store_batched");
+}
+
+extern "C" int aotb_ring_advance_batched(int* live, int* write, const int* store, int n, int rows, int cap_rows, int pinned_rows,
+                                         void* stream) {
+    AOTB_REQUIRE(live && write && store && n >= 1 && n <= 1024, "aotb_ring_advance_batched: bad args");
+    AOTB_REQUIRE(rows > 0 && pinned_rows >= 0 && (long long)pinned_rows + rows <= cap_rows &&
+                 (cap_rows - pinned_rows) % rows == 0,
+                 "aotb_ring_advance_batched: need rows > 0, pinned_rows + rows <= cap_rows and (cap_rows - pinned_rows) %% rows "
+                 "== 0 (got rows %d, cap_rows %d, pinned_rows %d)", rows, cap_rows, pinned_rows);
+    launch(ring_advance_batched_kernel, dim3(1), dim3(32 * ((n + 31) / 32)), 0, (cudaStream_t)stream, live, write, store, n, rows,
+           cap_rows, pinned_rows);
+    return check_launch("aotb_ring_advance_batched");
 }

@@ -427,7 +427,8 @@ __device__ __forceinline__ void mma_x3(float* d, const uint32_t* ah, const uint3
     mma16816(d, ah, bl[0], bl[1]);
 }
 
-__global__ void __launch_bounds__(256, 1) local_attn_mma_kernel(const LocalArgs p, const float* __restrict__ relv_t) {
+// One CTA of the tensor-core local attention over the map whose q / k / v / out rows `p` points at.
+__device__ __forceinline__ void local_attn_mma_cta(const LocalArgs& p, const float* __restrict__ relv_t) {
     pdl_sync();
     constexpr int TX = LTC_TX, HW = LTC_HW, LD = LTC_LD, SS = LTC_SS, NPOS = LTC_HH * LTC_HW;
     extern __shared__ __align__(16) float smem[];
@@ -642,6 +643,37 @@ __global__ void __launch_bounds__(256, 1) local_attn_mma_kernel(const LocalArgs 
             dst[1] = make_float4(o[0][2 * r + 1] * inv, o[1][2 * r + 1] * inv, o[2][2 * r + 1] * inv, o[3][2 * r + 1] * inv);
         }
     }
+}
+
+__global__ void __launch_bounds__(256, 1) local_attn_mma_kernel(const LocalArgs p, const float* __restrict__ relv_t) {
+    local_attn_mma_cta(p, relv_t);
+}
+
+// n maps of h x w pixels stacked along the rows: map b = blockIdx.z is rows [b h w, (b + 1) h w) of q, k, v and out.
+__global__ void __launch_bounds__(256, 1) local_attn_mma_batched_kernel(const LocalArgs p, const float* __restrict__ relv_t) {
+    const size_t r0 = (size_t)blockIdx.z * p.h * p.w;
+    LocalArgs pb = p;
+    pb.q += r0 * p.ldq;
+    pb.k += r0 * p.ldk;
+    pb.v += r0 * p.ldv;
+    pb.out += r0 * p.ldo;
+    local_attn_mma_cta(pb, relv_t);
+}
+
+static int launch_local_tc_batched(const LocalArgs& a, const float* relv_t, int n, cudaStream_t st) {
+    static bool configured = false;
+    if (!configured) {
+        cudaError_t e = cudaFuncSetAttribute(local_attn_mma_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)LTC_SMEM);
+        if (e != cudaSuccess) {
+            set_error("aotb_local_attention_tc_batched_f32: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+            return AOTB_ERR_CUDA;
+        }
+        configured = true;
+    }
+    dim3 grid(cdiv(a.h, LTC_TY) * cdiv(a.w, LTC_TX), a.H, n);
+    launch(local_attn_mma_batched_kernel, grid, dim3(256), LTC_SMEM, st, a, relv_t);
+    return check_launch("aotb_local_attention_tc_batched_f32");
 }
 
 static int launch_local_tc(const LocalArgs& a, const float* relv_t, cudaStream_t st) {
@@ -933,4 +965,21 @@ extern "C" int aotb_local_gated_tile_f32(const float* q, int ldq, const float* k
     a.relk_w = relk_w; a.relk_b = relk_b; a.relv = nullptr; a.out = out; a.ldo = ldo;
     a.h = h; a.w = w; a.H = 1; a.T = sqrtf(128.f);
     return launch_local_gated_tile(a, (cudaStream_t)stream);
+}
+
+// n maps of h x w pixels stacked along the rows of q, k, v and out (map b = rows [b h w, (b + 1) h w)); map b's output is bit
+// for bit aotb_local_attention_tc_f32 on its rows.
+extern "C" int aotb_local_attention_tc_batched_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                                                   const float* relk_w, const float* relk_b, const float* relv_t, float* out,
+                                                   int ldo, int h, int w, int H, int n, void* stream) {
+    AOTB_REQUIRE(q && k && v && relk_w && relk_b && relv_t && out && h > 0 && w > 0 && H > 0 && n >= 1 && n <= 65535,
+                 "aotb_local_attention_tc_batched_f32: bad args");
+    AOTB_REQUIRE(ldq % 4 == 0 && ldk % 4 == 0 && ldv % 4 == 0 && ldo % 4 == 0, "aotb_local_attention_tc_batched_f32: ld %% 4");
+    AOTB_REQUIRE(((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)relk_w | (uintptr_t)relv_t | (uintptr_t)out) % 16 == 0,
+                 "aotb_local_attention_tc_batched_f32: q, k, v, relk_w, relv_t and out must be 16-byte aligned");
+    LocalArgs a;
+    a.q = q; a.ldq = ldq; a.k = k; a.ldk = ldk; a.v = v; a.ldv = ldv;
+    a.relk_w = relk_w; a.relk_b = relk_b; a.relv = nullptr; a.out = out; a.ldo = ldo;
+    a.h = h; a.w = w; a.H = H; a.T = sqrtf(32.f);
+    return launch_local_tc_batched(a, relv_t, n, (cudaStream_t)stream);
 }

@@ -940,3 +940,110 @@ def gp_attention_tc_slots(Qp, Kp, Vp, N, Tk_dev, slots, slot_rows, part, exact=T
                                             _p(Mp), _p(Lp), int(slots), int(slot_rows),
                                             (1 if exact else 0) | (4 if LT_SPIN else 0), _st(stream)),
           "aotb_gp_attn_tc_slots_f16x2")
+
+
+# ------------------------------------------------------------------ several independent videos per launch (multi_video.py)
+def lt_attention_tc_batched(Qp, q_stride, Kp, Vp, kv_stride, n, N, Tk=0, Tk_dev=None, O=None, splits=1, exact=True,
+                            part=None, stream=None):
+    """n attentions in one launch ("tile" layout): problem b's queries are rows [b q_stride, b q_stride + N) of Qp [H, q_rows,
+    64], its keys / values rows [b kv_stride, b kv_stride + Tk_dev[b]) of Kp / Vp [H, kv_rows, 64] (Tk_dev int32 [n], or Tk
+    for all when None); O [n N, H*32] receives rows [b N, (b + 1) N).  With splits > 1, `part` = (Opart [splits, n N, H*32],
+    Mpart [splits, H, n N], Lpart [splits, H, n N]) and O receives their merge."""
+    H, q_rows, _ = Qp.shape
+    if splits > 1:
+        Op, Mp, Lp = part
+        _chk(Op, Mp, Lp)
+        if tuple(Op.shape) != (splits, n * N, H * 32) or tuple(Mp.shape) != (splits, H, n * N) or Lp.shape != Mp.shape:
+            raise AotbError(f"lt_attention_tc_batched: partials must be [{splits}, {n * N}, {H * 32}] and [{splits}, {H}, "
+                            f"{n * N}], got {tuple(Op.shape)}, {tuple(Mp.shape)}, {tuple(Lp.shape)}")
+    else:
+        Op = Mp = Lp = None
+    if Tk_dev is not None and (Tk_dev.dtype != torch.int32 or not Tk_dev.is_cuda or Tk_dev.numel() != n):
+        raise AotbError(f"lt_attention_tc_batched: Tk_dev must be an int32 CUDA tensor [{n}]")
+    if O is None or O.shape[0] != n * N:
+        raise AotbError(f"lt_attention_tc_batched: O must have {n * N} rows")
+    _chk(O)
+    check(lib().aotb_lt_attn_tc_batched_f16x2(Qp.data_ptr(), int(q_stride), q_rows, Kp.data_ptr(), Vp.data_ptr(),
+                                              int(kv_stride), Kp.shape[1], int(n), int(N), int(Tk),
+                                              Tk_dev.data_ptr() if Tk_dev is not None else None, H,
+                                              _p(O) if splits == 1 else None, O.stride(0), _p(Op), _p(Mp), _p(Lp), int(splits),
+                                              (1 if exact else 0) | (4 if LT_SPIN else 0), _st(stream)),
+          "aotb_lt_attn_tc_batched_f16x2")
+    if splits > 1:
+        attn_merge(Op, Mp, Lp, O, H, 32, stream=stream)
+    return O
+
+
+def local_attention_tc_batched(q, k, v, relk_w, relk_b, relv_t, out, h, w, H, n, stream=None):
+    """local_attention_tc over n h x w maps stacked along the rows of q, k, v and out ([n h w, ...] each)."""
+    _chk(q, k, v, relk_w, relk_b, relv_t, out)
+    if any(t.shape[0] != n * h * w for t in (q, k, v, out)):
+        raise AotbError(f"local_attention_tc_batched: q, k, v and out need {n} x {h * w} rows")
+    check(lib().aotb_local_attention_tc_batched_f32(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(relk_w),
+                                                    _p(relk_b), _p(relv_t), _p(out), out.stride(0), h, w, H, int(n),
+                                                    _st(stream)), "aotb_local_attention_tc_batched_f32")
+    return out
+
+
+def id_embed_runs_batched(masks, wp, bias, out, C, nid, ksize, stride, pad, ln_gamma=None, ln_beta=None, stream=None):
+    """id_embed_runs over n label maps masks [n, Hm, Wm] (contiguous) -> out [n ho wo, C]."""
+    if masks.dim() != 3 or not masks.is_contiguous():
+        raise AotbError(f"id_embed_runs_batched: masks must be contiguous [n, Hm, Wm], got {tuple(masks.shape)}")
+    n, Hm, Wm = masks.shape
+    ho, wo = (Hm + 2 * pad - ksize) // stride + 1, (Wm + 2 * pad - ksize) // stride + 1
+    _id_embed_check("id_embed_runs_batched", masks[0], wp, (ksize, ksize + 1, nid, C), bias, out[:ho * wo], C, ksize, stride,
+                    pad, ln_gamma, ln_beta)
+    if out.shape[0] != n * ho * wo:
+        raise AotbError(f"id_embed_runs_batched: out must have {n * ho * wo} rows, got {out.shape[0]}")
+    check(lib().aotb_id_embed_runs_batched_f32(_p(masks), n, Hm, Wm, _p(wp), _p(bias), _p(ln_gamma), _p(ln_beta), _p(out),
+                                               out.stride(0), C, nid, ksize, stride, pad, _st(stream)),
+          "aotb_id_embed_runs_batched_f32")
+    return out
+
+
+def _flags(name, t, n):
+    if t is None or not t.is_cuda or t.dtype != torch.int32 or t.numel() != n or not t.is_contiguous():
+        raise AotbError(f"{name} must be a contiguous int32 CUDA tensor [{n}]")
+    return t.data_ptr()
+
+
+def bank_ring_store_batched(k_src, v_src, k_bank, v_bank, k_packed, v_packed, write_dev, store_dev, n, cap_rows, stream=None):
+    """Bounded banks of n videos, stacked: video b's bank is rows [b cap_rows, (b + 1) cap_rows) of k_bank / v_bank [>= n
+    cap_rows, C] and of k_packed / v_packed [C / 32, >= n cap_rows, 64] (views may start at a video's first row: the chunk
+    stride is the tensor's).  Where store_dev[b] != 0, video b's rows [b rows, (b + 1) rows) of k_src / v_src [n rows, C] go to
+    row write_dev[b] of its bank (int32 CUDA tensors [n])."""
+    _chk(k_src, v_src, k_bank, v_bank)
+    rows = k_src.shape[0] // n
+    if k_src.shape[0] != n * rows or v_src.shape[0] != n * rows:
+        raise AotbError(f"bank_ring_store_batched: k_src and v_src need {n} equal blocks of rows")
+    head_rows = None
+    for name, src, bank, packed in (("k", k_src, k_bank, k_packed), ("v", v_src, v_bank, v_packed)):
+        if bank is not None and (bank.shape[0] < n * cap_rows or bank.shape[1] < src.shape[1]):
+            raise AotbError(f"bank_ring_store_batched: {name}_bank {tuple(bank.shape)} holds fewer than {n} banks of "
+                            f"{cap_rows} x {src.shape[1]}")
+        if packed is not None:
+            if packed.dtype != torch.float16 or not packed.is_cuda or packed.dim() != 3 or packed.shape[2] != 64 or \
+                    packed.stride(2) != 1 or packed.stride(1) != 64 or packed.shape[0] * 32 != src.shape[1] or \
+                    packed.shape[1] < n * cap_rows:
+                raise AotbError(f"bank_ring_store_batched: {name}_packed must be fp16 [{src.shape[1]} / 32, >= {n * cap_rows}, "
+                                f"64] with dense rows")
+            hr = packed.stride(0) // 64
+            if head_rows not in (None, hr):
+                raise AotbError("bank_ring_store_batched: the packed copies need one chunk stride")
+            head_rows = hr
+    check(lib().aotb_bank_ring_store_batched(_p(k_src), k_src.stride(0), k_src.shape[1], _p(v_src), v_src.stride(0),
+                                             v_src.shape[1], rows, int(n), _p(k_bank),
+                                             k_bank.stride(0) if k_bank is not None else 0, _p(v_bank),
+                                             v_bank.stride(0) if v_bank is not None else 0, _p(k_packed), _p(v_packed),
+                                             int(cap_rows), int(head_rows if head_rows is not None else n * cap_rows),
+                                             _flags("bank_ring_store_batched: write_dev", write_dev, n),
+                                             _flags("bank_ring_store_batched: store_dev", store_dev, n), _st(stream)),
+          "aotb_bank_ring_store_batched")
+
+
+def ring_advance_batched(live_dev, write_dev, store_dev, n, rows, cap_rows, pinned_rows, stream=None):
+    """ring_advance for each of n banks whose store_dev[b] != 0 (live_dev / write_dev / store_dev int32 CUDA tensors [n])."""
+    check(lib().aotb_ring_advance_batched(_flags("ring_advance_batched: live_dev", live_dev, n),
+                                          _flags("ring_advance_batched: write_dev", write_dev, n),
+                                          _flags("ring_advance_batched: store_dev", store_dev, n), int(n), int(rows),
+                                          int(cap_rows), int(pinned_rows), _st(stream)), "aotb_ring_advance_batched")

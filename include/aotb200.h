@@ -389,6 +389,33 @@ int aotb_ring_advance(int* live, int* write, int rows, int cap_rows, int pinned_
 int aotb_ring_select_usage(const int* live, int* write, float* U, int* A, int rows, int cap_rows, int pinned_rows,
                            void* stream);
 
+/* ---- several independent videos in one launch (MultiVideoInferEngine).  Each entry point runs n problems whose rows are
+ * stacked; problem b's result is bit for bit the one-problem entry point named beside it on problem b's rows.
+ *   aotb_lt_attn_tc_batched_f16x2  (aotb_lt_attn_tc_f16x2, "tile" layout): queries at rows b q_stride of Qp [H][q_rows][64],
+ *       keys / values at rows b kv_stride of Kp / Vp [H][kv_rows][64], live keys Tk_dev[b] (int32 [n]; null: Tk for all);
+ *       O [n N][ldo], or with splits > 1 partials Opart [splits][n N][H*32], Mpart / Lpart [splits][H][n N] for
+ *       aotb_attn_merge_f32 over n N rows.  One split count for all problems; exact bits 0 (exact) and 2 (spin).
+ *   aotb_local_attention_tc_batched_f32  (aotb_local_attention_tc_f32): map b = rows [b h w, (b + 1) h w) of q, k, v, out.
+ *   aotb_id_embed_runs_batched_f32  (aotb_id_embed_runs_f32): label maps mask [n][Hm][Wm], output rows [b ho wo, ...).
+ *   aotb_bank_ring_store_batched  (aotb_bank_ring_store): bank b = rows [b cap_rows, (b + 1) cap_rows) of every copy (the
+ *       packed copies' 32-channel chunks head_rows rows apart) stores source rows [b rows, (b + 1) rows) at write[b], only
+ *       when store[b] != 0.
+ *   aotb_ring_advance_batched  (aotb_ring_advance): live[b] / write[b] of every bank with store[b] != 0 (n <= 1024). */
+int aotb_lt_attn_tc_batched_f16x2(const void* Qp, int q_stride, int q_rows, const void* Kp, const void* Vp, int kv_stride,
+                                  int kv_rows, int n, int N, int Tk, const int* Tk_dev, int H, float* O, int ldo, float* Opart,
+                                  float* Mpart, float* Lpart, int splits, int exact, void* stream);
+int aotb_local_attention_tc_batched_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                                        const float* relk_w, const float* relk_b, const float* relv_t, float* out, int ldo,
+                                        int h, int w, int H, int n, void* stream);
+int aotb_id_embed_runs_batched_f32(const float* mask, int n, int Hm, int Wm, const float* wp, const float* bias,
+                                   const float* ln_gamma, const float* ln_beta, float* out, int ldo, int C, int nid, int ksize,
+                                   int stride, int pad, void* stream);
+int aotb_bank_ring_store_batched(const float* k_src, int ldk, int k_cols, const float* v_src, int ldv, int v_cols, int rows,
+                                 int n, float* k_bank, int ldkb, float* v_bank, int ldvb, void* k_packed, void* v_packed,
+                                 int cap_rows, int head_rows, const int* write, const int* store, void* stream);
+int aotb_ring_advance_batched(int* live, int* write, const int* store, int n, int rows, int cap_rows, int pinned_rows,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,0 +1,105 @@
+"""Aggregate frames/s of n independent videos: (a) MultiVideoInferEngine, one batched pass per frame; (b) n AOTInferEngines
+on concurrent streams through engine.fork_join; (c) the same n engines one after another.  Per step: propagate + decode +
+argmax + memory update, timed between CUDA events (every arm decodes stride-4 logits and runs the fused upsample + argmax
+kernel to the output size); the arms alternate in one session after an untimed pass each.
+Seeded random weights, 10 objects, long_term_mem_max 8, gap 5.  Prints one JSON line per (model, n, arm)."""
+import argparse
+import json
+import os
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--models", default="r50_aotl,aott")
+    ap.add_argument("--videos", default="1,2,4,8")
+    ap.add_argument("--frames", type=int, default=100)
+    ap.add_argument("--size", default="481,849")
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    from aot_benchmark_b200 import EngineConfig, build_vos_model
+    from aot_benchmark_b200 import engine as E
+    from aot_benchmark_b200.multi_video import MultiVideoInferEngine
+    from oracle import weights as OW
+    H, W = (int(s) for s in a.size.split(","))
+    out_size = (480, 854)
+    M, gap, objs = 8, 5, 10
+    card = torch.cuda.get_device_name(0)
+    rows = []
+    for name in a.models.split(","):
+        cfg = EngineConfig("fps", name)
+        model = build_vos_model(cfg.MODEL_VOS, cfg)
+        model.load_state_dict(OW.build_state_dict(name, seed=0))
+        model = model.cuda().eval()
+        g = torch.Generator(device="cuda").manual_seed(0)
+        frame = torch.randn(1, 3, H, W, device="cuda", generator=g)
+        mask = torch.randint(0, objs + 1, (1, 1, H, W), device="cuda", generator=g).float()
+        for n in (int(s) for s in a.videos.split(",")):
+            multi = MultiVideoInferEngine(model, max_videos=n, long_term_mem_max=M, long_term_mem_gap=gap)
+            singles = [E.AOTInferEngine(model, long_term_mem_gap=gap, long_term_mem_max=M) for _ in range(n)]
+            owner = type("Owner", (), {})()
+
+            def run_multi(T):
+                vids = [multi.open_video(frame, mask, objs) for _ in range(n)]
+                for _ in range(T):
+                    multi.propagate({v: frame for v in vids})
+                    labs = multi.decode_labels(out_size)
+                    multi.update_memory({v: torch.nn.functional.interpolate(labs[v][None].float(), size=(H, W),
+                                                                             mode="nearest") for v in vids})
+                for v in vids:
+                    multi.close_video(v)
+
+            def step_single(e):          # the same decode work as decode_labels: stride-4 logits, fused upsample + argmax
+                e.match_propogate_one_frame(frame)
+                e.decode_current_logits(None)
+                lab = e.aot_engines[0].predict_current_mask(out_size)
+                e.update_memory(torch.nn.functional.interpolate(lab[None].float(), size=(H, W), mode="nearest"))
+
+            def run_single(T, concurrent):
+                for e in singles:
+                    e.restart_engine()
+                    e.add_reference_frame(frame, mask, obj_nums=[objs], frame_step=0)
+                if concurrent:
+                    for _ in range(T):
+                        E.fork_join(owner, singles, lambda i, e: step_single(e))
+                else:
+                    for e in singles:
+                        for _ in range(T):
+                            step_single(e)
+
+            arms = {"a_multi": run_multi, "b_streams": lambda T: run_single(T, True),
+                    "c_sequential": lambda T: run_single(T, False)}
+            with torch.no_grad():
+                for fn in arms.values():
+                    fn(3)                                  # untimed: captures, allocations
+                torch.cuda.synchronize()
+                times = {k: [] for k in arms}
+                for _ in range(2):
+                    for k, fn in arms.items():
+                        torch.cuda.reset_peak_memory_stats()
+                        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                        e0.record()
+                        fn(a.frames)
+                        e1.record()
+                        torch.cuda.synchronize()
+                        times[k].append((e0.elapsed_time(e1), torch.cuda.max_memory_allocated() / 2 ** 30))
+            for k, v in times.items():
+                best = min(t for t, _ in v)
+                r = dict(model=name, n=n, arm=k, frames=a.frames, fps=round(n * a.frames / (best / 1e3), 1),
+                         ms_per_step=round(best / a.frames, 3), peak_gib=round(max(m for _, m in v), 2), card=card)
+                print(json.dumps(r), flush=True)
+                rows.append(r)
+            del multi, singles
+            torch.cuda.empty_cache()
+    if a.out:
+        os.makedirs(os.path.dirname(a.out), exist_ok=True)
+        with open(a.out, "w") as f:
+            json.dump(rows, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
