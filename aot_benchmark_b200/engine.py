@@ -17,6 +17,7 @@ Training (AOTEngine.forward, aot_engine.py:33-108) is a "next" row of SURVEY 8(f
 """
 from __future__ import annotations
 
+import contextlib
 import functools
 import math
 
@@ -591,6 +592,147 @@ class _Encoder:
 
 
 # =====================================================================================
+# per-frame network body shared by AOTEngine and MultiVideoInferEngine: n maps stacked in the rows of one workspace
+# =====================================================================================
+@contextlib.contextmanager
+def _lt_probe(on, Q, Tk, C):
+    """With LT_PROBE set and `on`: CUDA events around the launches of the block and its FLOPs (4 N Tk C) appended."""
+    probe = LT_PROBE if on else None
+    if probe is None:
+        yield
+        return
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    yield
+    e1.record()
+    probe.append((e0, e1, 4.0 * Q.shape[0] * Tk * C))
+
+
+def _static_buf(bufs, key, shape, device):
+    """bufs[(key, shape)], an fp32 buffer allocated on first use and kept: bodies captured for several shapes (one per
+    video count n) each keep reading their own."""
+    t = bufs.get((key, shape))
+    if t is None:
+        t = bufs[(key, shape)] = torch.empty(shape, dtype=torch.float32, device=device)
+    return t
+
+
+def _split_partials(bufs, splits, rows, H, dv, device, cap_rows=None):
+    """Split-KV partials (O [splits, rows, dv], m [splits, H, rows], l [splits, H, rows]): contiguous views of three
+    flat fp32 allocations per split count, kept in bufs and sized for cap_rows (default rows) query rows, so bodies over any
+    rows <= cap_rows read memory that lives as long as bufs."""
+    views = bufs.get((splits, rows))
+    if views is None:
+        flat = bufs.get(splits)
+        if flat is None:
+            cap = cap_rows or rows
+            flat = bufs[splits] = [torch.empty(splits * cap * c, dtype=torch.float32, device=device)
+                                   for c in (dv, H, H)]
+        O, m, l = flat
+        nM = splits * H * rows
+        views = bufs[(splits, rows)] = (O[:splits * rows * dv].view(splits, rows, dv), m[:nM].view(splits, H, rows),
+                                        l[:nM].view(splits, H, rows))
+    return views
+
+
+def _aot_lstt_buffers(rows, C, L, device):
+    """The AOT LSTT's fp32 activations over `rows` token rows, by name (curr_Q, curr_V, st_K, st_V: per-layer lists)."""
+    f = lambda c: torch.empty((rows, c), dtype=torch.float32, device=device)
+    out = {k: f(m * C) for k, m in (("id_emb", 1), ("x", 1), ("ln", 1), ("ln_pos", 1), ("qk", 2), ("v", 1), ("core", 2),
+                                    ("tmp", 1), ("ff", 4), ("ff2", 4), ("cat", L + 1))}
+    out.update((k, [f(C) for _ in range(L)]) for k in ("curr_Q", "curr_V", "st_K", "st_V"))
+    return out
+
+
+def _fuse_layer(Lw, cQ, cV, id_emb, tmp, K, V, st):
+    """fuse_key_value_id (transformer.py:364-367) of one layer: K = curr_K, V = linear_V(curr_V + id)."""
+    ops.eltwise(ops.EW_ADD, cV, id_emb, tmp, stream=st)
+    ops.linear(tmp, Lw.linV_w, Lw.linV_b, V, stream=st)
+    ops.eltwise(ops.EW_COPY, cQ, None, K, stream=st)
+
+
+def aot_fuse_memories(P, a, id_emb, K, V, st):
+    """update_short_term_memory core (aot_engine.py:315-332) over the rows of workspace `a`: the short-term K[li] /
+    V[li] of every layer from its curr_Q / curr_V and the ID embedding."""
+    for li in range(P.L):
+        _fuse_layer(P.layers[li], a.curr_Q[li], a.curr_V[li], id_emb, a.tmp, K[li], V[li], st)
+
+
+def aot_lstt(P, a, proj, pos, hw, n, st_K, st_V, id_emb, attend_own, attend_bank, local, st):
+    """The AOT LSTT (transformer.py:321-359) over n maps of hw = (h, w) tokens stacked in the rows of workspace `a`
+    (x, ln, ln_pos, qk, v, core, tmp, ff, ff2, cat, curr_Q, curr_V sliced to those rows, and the groupnorm workspace
+    gn_ws for n maps); proj: their projected 16x features, pos: the position table over the same rows.  id_emb None: a
+    propagated frame, whose long-term step reads the bank; else a reference frame, whose short-term K / V (st_K, st_V)
+    are fused first and are its long-term memory.  The engine's hooks launch the attention steps:
+      attend_own(Q, K, V, out, st, long_term)   over the frame's own K / V: the self-attention, and (long_term=True) the
+                                                reference frame's long-term step
+      attend_bank(li, Q, out, st)               the long-term step over layer li's bank
+      local(li, Q, K, V, out, st)               the short-term local attention"""
+    C = P.C
+    h, w = hw
+    x = a.x
+    ops.eltwise(ops.EW_COPY, proj, None, x, stream=st)
+    ops.eltwise(ops.EW_COPY, proj, None, a.cat[:, :C], stream=st)
+    for li in range(P.L):
+        Lw = P.layers[li]
+        # 1) self-attention (transformer.py:321-326)
+        ops.layernorm(x, Lw.norm1[0], Lw.norm1[1], a.ln, add=pos, out2=a.ln_pos, stream=st)
+        ops.linear(a.ln_pos, Lw.sa_qk_w, Lw.sa_qk_b, a.qk, stream=st)
+        ops.linear(a.ln, Lw.sa_v_w, Lw.sa_v_b, a.v, stream=st)
+        attend_own(a.qk[:, :C], a.qk[:, C:], a.v, a.core[:, :C], st, False)
+        ops.linear(a.core[:, :C], Lw.sa_proj_w, Lw.sa_proj_b, x, res=x, stream=st)
+        # 2) long + short term (transformer.py:329-352)
+        cQ, cV = a.curr_Q[li], a.curr_V[li]
+        ops.layernorm(x, Lw.norm2[0], Lw.norm2[1], cV, stream=st)
+        ops.linear(cV, Lw.linQ_w, Lw.linQ_b, cQ, stream=st)
+        if id_emb is not None:
+            _fuse_layer(Lw, cQ, cV, id_emb, a.tmp, st_K[li], st_V[li], st)
+            attend_own(cQ, st_K[li], st_V[li], a.core[:, :C], st, True)
+        else:
+            attend_bank(li, cQ, a.core[:, :C], st)
+        local(li, cQ, st_K[li], st_V[li], a.core[:, C:], st)
+        ops.linear(a.core, Lw.lst_proj_w, Lw.lst_proj_b, x, res=x, stream=st)
+        # 3) feed-forward (transformer.py:354-359, basic.py:27-35)
+        ops.layernorm(x, Lw.norm3[0], Lw.norm3[1], a.ln, stream=st)
+        ops.linear(a.ln, Lw.lin1_w, Lw.lin1_b, a.ff, stream=st)
+        ops.groupnorm(a.ff.view(n, h * w, 4 * C), Lw.gn[0], Lw.gn[1], a.ff.view(n, h * w, 4 * C), 32, A_GELU, a.gn_ws,
+                      stream=st)
+        ops.dwconv(a.ff.view(n, h, w, 4 * C), Lw.dw_w, None, a.ff2.view(n, h, w, 4 * C), K=5, pad=2, stream=st)
+        ops.linear(a.ff2, Lw.lin2_w, Lw.lin2_b, x, res=x, stream=st)
+        # decoder norms (transformer.py:124-135) written straight into the decoder input
+        ops.layernorm(x, Lw.dec_norm[0], Lw.dec_norm[1], a.cat[:, (li + 1) * C:(li + 2) * C], stream=st)
+
+
+def fpn_decode(P, cat_nhwc, x4, x8, x16, dbuf, gn_ws, st):
+    """The FPN decoder (fpn.py:34-58) over B = x4.shape[0] images: cat_nhwc [B, h, w, c] the LSTT output, x4 / x8 / x16
+    the encoder maps -> logits [B, h4, w4, 11] (NHWC).  Every intermediate map is a static buffer of the dict dbuf."""
+    D = P.dec
+    B = x4.shape[0]
+    buf = lambda key, x, c: _static_buf(dbuf, key, (B, x.shape[1], x.shape[2], c), x.device)
+
+    def conv_gn(x, blk, key, k, pad):
+        o = buf(key, x, blk.cout)
+        ops.conv2d(x, blk.w, blk.b, o, KH=k, KW=k, pad=pad, stream=st)
+        ov = o.view(B, -1, blk.cout)
+        ops.groupnorm(ov, blk.gn[0], blk.gn[1], ov, 8, A_RELU, gn_ws, stream=st)
+        return o
+
+    x = conv_gn(cat_nhwc, D.conv_in, "in", 1, 0)
+    a = buf("a16", x16, D.adapter_16x.cout)
+    ops.conv2d(x16, D.adapter_16x.w, D.adapter_16x.b, a, res=x, stream=st)
+    x = conv_gn(a, D.conv_16x, "c16", 3, 1)
+    for xs, tag, ad, cv in ((x8, "8", D.adapter_8x, D.conv_8x), (x4, "4", D.adapter_4x, D.conv_4x)):
+        up = buf("up" + tag, xs, x.shape[3])
+        ops.bilinear(x, up, P.align_corners, stream=st)
+        a = buf("a" + tag, xs, ad.cout)
+        ops.conv2d(xs, ad.w, ad.b, a, res=up, stream=st)
+        x = conv_gn(a, cv, "c" + tag, 3, 1)
+    lg = buf("logit", x, D.conv_out.cout)
+    ops.conv2d(x, D.conv_out.w, D.conv_out.b, lg, stream=st)
+    return lg
+
+
+# =====================================================================================
 # single engine (<= max_obj_num objects)
 # =====================================================================================
 class AOTEngine(nn.Module):
@@ -730,25 +872,15 @@ class AOTEngine(nn.Module):
         ws = type("WS", (), {})()
         ws.N = N
         ws.gn_ws = ops.groupnorm_workspace(1, 32, dev)
-        ws.id_emb = f(N, C)
         if not P.deaot:
-            ws.x = f(N, C)
-            ws.ln = f(N, C)
-            ws.ln_pos = f(N, C)
-            ws.qk = f(N, 2 * C)
-            ws.v = f(N, C)
-            ws.core = f(N, 2 * C)
-            ws.tmp = f(N, C)
-            ws.ff = f(N, 4 * C)
-            ws.ff2 = f(N, 4 * C)
-            ws.cat = f(N, (L + 1) * C)
-            self.curr_Q = [f(N, C) for _ in range(L)]
-            self.curr_V = [f(N, C) for _ in range(L)]
-            self.st_K = [f(N, C) for _ in range(L)]
-            self.st_V = [f(N, C) for _ in range(L)]
+            bufs = _aot_lstt_buffers(N, C, L, dev)
+            self.st_K, self.st_V = bufs.pop("st_K"), bufs.pop("st_V")     # the live slot: _commit_short_slot moves it
+            vars(ws).update(bufs)
+            self.curr_Q, self.curr_V = ws.curr_Q, ws.curr_V
             self._kdim, self._vdim = C, C
         else:
             d = C // 2
+            ws.id_emb = f(N, C)
             ws.xz = f(N, 2 * C)
             ws.ln = f(N, C)
             ws.qv = f(N, d + 2 * C)
@@ -1199,90 +1331,55 @@ class AOTEngine(nn.Module):
     # ------------------------------------------------------------------ LSTT (AOT)
     def _lstt_forward(self, embs, id_emb, st):
         P = self._plan()
-        ws = self._ws
-        N, C, H = self.enc_hw, P.C, P.H
-        h, w = self.enc_size_2d
-        d = C // H
-        proj = embs.nhwc[-1].view(N, C)
-        ops.eltwise(ops.EW_COPY, proj, None, ws.x, stream=st)
-        ops.eltwise(ops.EW_COPY, proj, None, ws.cat[:, :C], stream=st)
-        x = ws.x
-        is_ref = id_emb is not None
-        if is_ref:
-            stK, stV = self._next_short_slot()
-        else:
-            stK, stV = self.st_K, self.st_V
-        for li in range(P.L):
-            Lw = P.layers[li]
-            # 1) self-attention (transformer.py:321-326)
-            ops.layernorm(x, Lw.norm1[0], Lw.norm1[1], ws.ln, add=self.pos_emb, out2=ws.ln_pos, stream=st)
-            ops.linear(ws.ln_pos, Lw.sa_qk_w, Lw.sa_qk_b, ws.qk, stream=st)
-            ops.linear(ws.ln, Lw.sa_v_w, Lw.sa_v_b, ws.v, stream=st)
-            if self._tc:
-                self._tc_attention(ws.qk[:, :C], ws.qk[:, C:], ws.v, None, None, N, ws.core[:, :C], st)
-            else:
-                ops.attention(ws.qk[:, :C], ws.qk[:, C:], ws.v, ws.core[:, :C], H, d, d, Tk=N, stream=st)
-            ops.linear(ws.core[:, :C], Lw.sa_proj_w, Lw.sa_proj_b, x, res=x, stream=st)
-            # 2) long + short term (transformer.py:329-352)
-            cQ, cV = self.curr_Q[li], self.curr_V[li]
-            ops.layernorm(x, Lw.norm2[0], Lw.norm2[1], cV, stream=st)
-            ops.linear(cV, Lw.linQ_w, Lw.linQ_b, cQ, stream=st)
-            if is_ref:
-                ops.eltwise(ops.EW_ADD, cV, id_emb, ws.tmp, stream=st)
-                ops.linear(ws.tmp, Lw.linV_w, Lw.linV_b, stV[li], stream=st)      # fuse_key_value_id :364-367
-                ops.eltwise(ops.EW_COPY, cQ, None, stK[li], stream=st)
-                gK, gV, Tk = stK[li], stV[li], N
-            else:
-                gK, gV, Tk = self.bank_K[li], self.bank_V[li], self.bank_len
-            self._long_term_attention(li, cQ, gK, gV, Tk, ws.core[:, :C], st)
-            if d == 32 and LOCAL_IMPL in ops.LOCAL_KERNELS:
-                with ops.local_kernel(LOCAL_IMPL):
-                    ops.local_attention_tile(cQ, stK[li], stV[li], Lw.relk_w, Lw.relk_b, Lw.relv_t, ws.core[:, C:], h, w,
-                                             H, stream=st)
-            else:
-                ops.local_attention(cQ, stK[li], stV[li], Lw.relk_w, Lw.relk_b, Lw.relv, ws.core[:, C:], h, w, H, d, d,
-                                    stream=st)
-            ops.linear(ws.core, Lw.lst_proj_w, Lw.lst_proj_b, x, res=x, stream=st)
-            # 3) feed-forward (transformer.py:354-359, basic.py:27-35)
-            ops.layernorm(x, Lw.norm3[0], Lw.norm3[1], ws.ln, stream=st)
-            ops.linear(ws.ln, Lw.lin1_w, Lw.lin1_b, ws.ff, stream=st)
-            ops.groupnorm(ws.ff.view(1, N, 4 * C), Lw.gn[0], Lw.gn[1], ws.ff.view(1, N, 4 * C), 32, A_GELU, ws.gn_ws,
-                          stream=st)
-            ops.dwconv(ws.ff.view(1, h, w, 4 * C), Lw.dw_w, None, ws.ff2.view(1, h, w, 4 * C), K=5, pad=2, stream=st)
-            ops.linear(ws.ff2, Lw.lin2_w, Lw.lin2_b, x, res=x, stream=st)
-            # decoder norms (transformer.py:124-135) written straight into the decoder input
-            ops.layernorm(x, Lw.dec_norm[0], Lw.dec_norm[1], ws.cat[:, (li + 1) * C:(li + 2) * C], stream=st)
-        if is_ref:
+        stK, stV = (self.st_K, self.st_V) if id_emb is None else self._next_short_slot()
+        aot_lstt(P, self._ws, embs.nhwc[-1].view(self.enc_hw, P.C), self.pos_emb, self.enc_size_2d, 1, stK, stV, id_emb,
+                 self._attend_own, self._attend_bank, self._local_attention, st)
+        if id_emb is not None:
             self._commit_short_slot(stK, stV)
         self._have_lstt = True
 
-    def _long_term_attention(self, li, Q, K, V, Tk, out, st):
+    def _attend_own(self, Q, K, V, out, st, long_term):
+        """softmax(Q K^T / T) V over the frame's own K / V: the self-attention, or (long_term) a reference frame's
+        long-term step (transformer.py:337-341), which LT_PROBE times."""
         P = self._plan()
         d = P.C // P.H
-        probe = LT_PROBE
-        use_tc = self._tc and (K is self.bank_K[li])
-        if use_tc:
+        with _lt_probe(long_term, Q, self.enc_hw, P.C):
+            if self._tc:
+                self._tc_attention(Q, K, V, None, None, self.enc_hw, out, st)
+            else:
+                ops.attention(Q, K, V, out, P.H, d, d, Tk=self.enc_hw, stream=st)
+
+    def _attend_bank(self, li, Q, out, st):
+        """The long-term step of a propagated frame over layer li's bank."""
+        P = self._plan()
+        d = P.C // P.H
+        if self._tc:
             ops.tc_pack_rows(Q, self._ws.Qp, 0, div=math.sqrt(d), stream=st)      # Q / T (attention.py:82)
-        if probe is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-        if use_tc and self.kv_shard is not None:
-            self._sharded_attention(li, out, st)
-        elif self.kv_shard is not None and K is self.bank_K[li]:
+        elif self.kv_shard is not None:
             raise ops.AotbError("sharded long-term bank needs the tensor-core attention kernel (8 heads x 32); this model's "
                                 "head shape runs on the fp32 kernel, which has no partial (m, l, O) outputs")
-        elif use_tc and self._usage():
-            self._usage_attention(li, self._ws.Qp, self.bank_Kp[li], self.bank_Vp[li], out, st)
-        elif use_tc:
-            self._tc_attention(None, None, None, self.bank_Kp[li], self.bank_Vp[li], Tk, out, st, Tk_dev=self.tk_dev)
-        elif self._tc:
-            self._tc_attention(Q, K, V, None, None, Tk, out, st)     # reference frame: Tk = N, own K/V
+        with _lt_probe(True, Q, self.bank_len, P.C):
+            if not self._tc:
+                ops.attention(Q, self.bank_K[li], self.bank_V[li], out, P.H, d, d, Tk=self.bank_len, Tk_dev=self.tk_dev,
+                              stream=st)
+            elif self.kv_shard is not None:
+                self._sharded_attention(li, out, st)
+            elif self._usage():
+                self._usage_attention(li, self._ws.Qp, self.bank_Kp[li], self.bank_Vp[li], out, st)
+            else:
+                self._tc_attention(None, None, None, self.bank_Kp[li], self.bank_Vp[li], self.bank_len, out, st,
+                                   Tk_dev=self.tk_dev)
+
+    def _local_attention(self, li, Q, K, V, out, st):
+        P = self._plan()
+        Lw = P.layers[li]
+        h, w = self.enc_size_2d
+        d = P.C // P.H
+        if d == 32 and LOCAL_IMPL in ops.LOCAL_KERNELS:
+            with ops.local_kernel(LOCAL_IMPL):
+                ops.local_attention_tile(Q, K, V, Lw.relk_w, Lw.relk_b, Lw.relv_t, out, h, w, P.H, stream=st)
         else:
-            ops.attention(Q, K, V, out, P.H, d, d, Tk=Tk, Tk_dev=self.tk_dev if K is self.bank_K[li] else None,
-                          stream=st)
-        if probe is not None:
-            e1.record()
-            probe.append((e0, e1, 4.0 * Q.shape[0] * Tk * P.C))
+            ops.local_attention(Q, K, V, Lw.relk_w, Lw.relk_b, Lw.relv, out, h, w, P.H, d, d, stream=st)
 
     def _tc_attention(self, Q, K, V, Kp, Vp, Tk, out, st, Tk_dev=None):
         """softmax(Q K^T / T) V on the tensor-core kernel.  Q/K/V fp32 [rows, C] are packed into the split-fp16
@@ -1298,13 +1395,7 @@ class AOTEngine(nn.Module):
             ops.tc_pack_rows(V, ws.saVp, 0, stream=st)
             Kp, Vp = ws.saKp, ws.saVp
         splits = lt_splits(N, P.H, Tk)
-        part = None
-        if splits > 1:
-            part = ws.part.get(splits)
-            if part is None:
-                fz = lambda *s: torch.empty(s, dtype=torch.float32, device=out.device)
-                part = (fz(splits, N, P.C), fz(splits, P.H, N), fz(splits, P.H, N))
-                ws.part[splits] = part
+        part = _split_partials(ws.part, splits, N, P.H, P.C, out.device) if splits > 1 else None
         exact = LT_IMPL == "tc_exact" and self.precision == "fp32"
         ops.lt_attention_tc(ws.Qp, Kp, Vp, N, Tk, O=out, Tk_dev=Tk_dev, splits=splits, exact=exact, part=part, stream=st)
 
@@ -1422,60 +1513,14 @@ class AOTEngine(nn.Module):
         self.st_K, self.st_V = self._st_ring[0]
 
     def _fuse_memories(self, id_emb, st):
-        """update_short_term_memory core (aot_engine.py:315-332): K = curr_K, V = linear_V(curr_V + id)."""
-        P = self._plan()
-        ws = self._ws
         K, V = self._next_short_slot()
-        for li in range(P.L):
-            Lw = P.layers[li]
-            ops.eltwise(ops.EW_ADD, self.curr_V[li], id_emb, ws.tmp, stream=st)
-            ops.linear(ws.tmp, Lw.linV_w, Lw.linV_b, V[li], stream=st)
-            ops.eltwise(ops.EW_COPY, self.curr_Q[li], None, K[li], stream=st)
+        aot_fuse_memories(self._plan(), self._ws, id_emb, K, V, st)
         self._commit_short_slot(K, V, reset=False)
 
-    # ------------------------------------------------------------------ decoder (fpn.py:34-58)
-    def _dbuf(self, key, shape):
-        b = self._dec_bufs.get(key)
-        if b is None or tuple(b.shape) != tuple(shape):
-            b = torch.empty(shape, dtype=torch.float32, device=self._plan().device)
-            self._dec_bufs[key] = b
-        return b
-
     def _decode(self, st):
-        P = self._plan()
-        D = P.dec
-        ws = self._ws
-        ac = P.align_corners
         x4, x8, x16, _ = self.curr_enc_embs.nhwc
-        h, w = self.enc_size_2d
-        C = P.C
-        gws = ws.gn_ws
-
-        def conv_gn(x, blk, key, k, pad, res=None):
-            o = self._dbuf(key, (1, x.shape[1], x.shape[2], blk.cout))
-            ops.conv2d(x, blk.w, blk.b, o, KH=k, KW=k, pad=pad, stream=st)
-            ov = o.view(1, -1, blk.cout)
-            ops.groupnorm(ov, blk.gn[0], blk.gn[1], ov, 8, A_RELU, gws, stream=st)
-            return o
-
-        cat = ws.cat.view(1, h, w, -1)
-        x = conv_gn(cat, D.conv_in, "in", 1, 0)
-        a = self._dbuf("a16", (1, h, w, D.adapter_16x.cout))
-        ops.conv2d(x16, D.adapter_16x.w, D.adapter_16x.b, a, res=x, stream=st)
-        x = conv_gn(a, D.conv_16x, "c16", 3, 1)
-        up = self._dbuf("up8", (1, x8.shape[1], x8.shape[2], x.shape[3]))
-        ops.bilinear(x, up, ac, stream=st)
-        a = self._dbuf("a8", (1, x8.shape[1], x8.shape[2], D.adapter_8x.cout))
-        ops.conv2d(x8, D.adapter_8x.w, D.adapter_8x.b, a, res=up, stream=st)
-        x = conv_gn(a, D.conv_8x, "c8", 3, 1)
-        up = self._dbuf("up4", (1, x4.shape[1], x4.shape[2], x.shape[3]))
-        ops.bilinear(x, up, ac, stream=st)
-        a = self._dbuf("a4", (1, x4.shape[1], x4.shape[2], D.adapter_4x.cout))
-        ops.conv2d(x4, D.adapter_4x.w, D.adapter_4x.b, a, res=up, stream=st)
-        x = conv_gn(a, D.conv_4x, "c4", 3, 1)
-        lg = self._dbuf("logit", (1, x.shape[1], x.shape[2], D.conv_out.cout))
-        ops.conv2d(x, D.conv_out.w, D.conv_out.b, lg, stream=st)
-        return lg
+        return fpn_decode(self._plan(), self._ws.cat.view(1, *self.enc_size_2d, -1), x4, x8, x16, self._dec_bufs,
+                          self._ws.gn_ws, st)
 
     @_in_precision
     def decode_current_logits(self, output_size=None):
@@ -1635,12 +1680,7 @@ class DeAOTEngine(AOTEngine):
             ops.tc_pack_rows(V, ws.gpSaV, 0, stream=st)
             Kp, Vp = ws.gpSaK, ws.gpSaV
         splits = self._gp_splits(Tk)
-        part = None
-        if splits > 1:
-            part = ws.gp_part.get(splits)
-            if part is None:
-                fz = lambda *s: torch.empty(s, dtype=torch.float32, device=out.device)
-                part = ws.gp_part[splits] = (fz(splits, N, out.shape[1]), fz(splits, 1, N), fz(splits, 1, N))
+        part = _split_partials(ws.gp_part, splits, N, 1, out.shape[1], out.device) if splits > 1 else None
         ops.gp_attention_tc(ws.gpQp, Kp, Vp, N, Tk, O=out, Tk_dev=Tk_dev, splits=splits, exact=self.precision == "fp32",
                             part=part, stream=st)
 

@@ -9,6 +9,7 @@ allocated once per (geometry, S, M), so every launch covers exactly n videos and
 from __future__ import annotations
 
 import math
+import types
 
 import torch
 
@@ -209,8 +210,8 @@ class MultiVideoInferEngine:
         h4, w4, NC = lg.shape[1], lg.shape[2], lg.shape[3]
         self._last_lowres, out = [], {}
         for b, s in enumerate(self._slots):
-            lo = self._dbuf(("lo", b), (1, NC, h4, w4))
-            up = None if size is None else self._dbuf(("out", b), (1, NC) + size)
+            lo = E._static_buf(self._pool.dec, ("lo", b), (1, NC, h4, w4), lg.device)
+            up = None if size is None else E._static_buf(self._pool.dec, ("out", b), (1, NC) + size, lg.device)
             ops.logits_postproc(lg[b:b + 1], lo, up, s["obj"], self._P.align_corners, stream=st)
             self._last_lowres.append(lo)
             out[s["vid"]] = lo if up is None else up
@@ -256,7 +257,8 @@ class MultiVideoInferEngine:
             P, N = self._P, self._N
             ops.id_embed_runs_batched(pl.mask[:n], P.id_wp, P.id_b, pl.id_emb[:n * N], P.C, P.nid, P.id_k, P.id_stride,
                                       P.id_pad, stream=s2)
-            self._fuse(0, n, s2)
+            a = self._rows(0, n)
+            E.aot_fuse_memories(P, a, a.id_emb, a.st_K, a.st_V, s2)
             self._store(0, n, s2)
         self.graphs.run(("upd", n), body)
         for s, f in zip(self._slots, flags):
@@ -330,12 +332,8 @@ class MultiVideoInferEngine:
         pl.tk = torch.zeros(S, dtype=torch.int32, device=dev)
         pl.wr = torch.zeros(S, dtype=torch.int32, device=dev)
         R = S * N
-        pl.id_emb, pl.x, pl.ln, pl.ln_pos, pl.v, pl.tmp = (f(R, C) for _ in range(6))
-        pl.qk, pl.core = f(R, 2 * C), f(R, 2 * C)
-        pl.ff, pl.ff2 = f(R, 4 * C), f(R, 4 * C)
-        pl.cat = f(R, (L + 1) * C)
-        pl.curr_Q, pl.curr_V = [f(R, C) for _ in range(L)], [f(R, C) for _ in range(L)]
-        pl.st_K, pl.st_V = [f(R, C) for _ in range(L)], [f(R, C) for _ in range(L)]
+        pl.lstt = E._aot_lstt_buffers(R, C, L, dev)
+        vars(pl).update(pl.lstt)
         pl.bank_K, pl.bank_V = [f(S * M * N, C) for _ in range(L)], [f(S * M * N, C) for _ in range(L)]
         pl.bank_Kp, pl.bank_Vp = [hz(P.H, S * M * N, 64) for _ in range(L)], [hz(P.H, S * M * N, 64) for _ in range(L)]
         pl.Qp, pl.saKp, pl.saVp = hz(P.H, R, 64), hz(P.H, R, 64), hz(P.H, R, 64)
@@ -351,81 +349,47 @@ class MultiVideoInferEngine:
             raise ValueError(f"expected a label map of the network input size {self._geom}, got {tuple(mask.shape)}")
         ops.eltwise(ops.EW_COPY, m.float().contiguous(), None, self._pool.mask[b], stream=st)
 
-    def _parts(self, splits, rows):
-        """Split-KV partials of `splits` splits over `rows` query rows: views of one allocation per split count, so a graph
-        body for any n reads memory that lives as long as the pool."""
-        pl, H, C = self._pool, self._P.H, self._P.C
-        flat = pl.part.get(splits)
-        if flat is None:
-            R = self.max_videos * self._N
-            flat = pl.part[splits] = torch.empty(splits * R * (C + 2 * H), dtype=torch.float32, device=pl.x.device)
-        nO, nM = splits * rows * C, splits * H * rows
-        return (flat[:nO].view(splits, rows, C), flat[nO:nO + nM].view(splits, H, rows),
-                flat[nO + nM:nO + 2 * nM].view(splits, H, rows))
-
     def _attention(self, Q, Kp, Vp, kv_stride, n, Tk, Tk_dev, out, splits, st):
         P, N = self._P, self._N
         pl = self._pool
         ops.tc_pack_rows(Q, pl.Qp, 0, div=math.sqrt(P.C // P.H), stream=st)
         exact = E.LT_IMPL == "tc_exact" and self.precision == "fp32"
+        part = E._split_partials(pl.part, splits, n * N, P.H, P.C, pl.x.device, cap_rows=self.max_videos * N) \
+            if splits > 1 else None
         ops.lt_attention_tc_batched(pl.Qp, N, Kp, Vp, kv_stride, n, N, Tk=Tk, Tk_dev=Tk_dev, O=out, splits=splits,
-                                    exact=exact, part=self._parts(splits, n * N) if splits > 1 else None, stream=st)
+                                    exact=exact, part=part, stream=st)
 
     # ------------------------------------------------------------------ batched bodies (rows of slots b .. b + n - 1)
-    def _lstt(self, b, n, proj, st, ref, splits=None):
-        """AOTEngine._lstt_forward over slots [b, b + n): ref = the reference-frame form (the frame's own K / V as long-term
-        memory, short-term memory written), else the propagation form over the slots' banks."""
-        P, pl, N = self._P, self._pool, self._N
-        C, H = P.C, P.H
-        h, w = self._hw
-        r = slice(b * N, (b + n) * N)
-        R = n * N
-        x, ln, ln_pos, qk, v, core, tmp = (t[r] for t in (pl.x, pl.ln, pl.ln_pos, pl.qk, pl.v, pl.core, pl.tmp))
-        ff, ff2, cat = pl.ff[r], pl.ff2[r], pl.cat[r]
-        ops.eltwise(ops.EW_COPY, proj, None, x, stream=st)
-        ops.eltwise(ops.EW_COPY, proj, None, cat[:, :C], stream=st)
-        sa_splits = E.lt_splits(R, H, N)
-        for li in range(P.L):
-            Lw = P.layers[li]
-            stK, stV = pl.st_K[li][r], pl.st_V[li][r]
-            ops.layernorm(x, Lw.norm1[0], Lw.norm1[1], ln, add=pl.pos[:R], out2=ln_pos, stream=st)
-            ops.linear(ln_pos, Lw.sa_qk_w, Lw.sa_qk_b, qk, stream=st)
-            ops.linear(ln, Lw.sa_v_w, Lw.sa_v_b, v, stream=st)
-            ops.tc_pack_rows(qk[:, C:], pl.saKp, 0, stream=st)
-            ops.tc_pack_rows(v, pl.saVp, 0, stream=st)
-            self._attention(qk[:, :C], pl.saKp, pl.saVp, N, n, N, None, core[:, :C], sa_splits, st)
-            ops.linear(core[:, :C], Lw.sa_proj_w, Lw.sa_proj_b, x, res=x, stream=st)
-            cQ, cV = pl.curr_Q[li][r], pl.curr_V[li][r]
-            ops.layernorm(x, Lw.norm2[0], Lw.norm2[1], cV, stream=st)
-            ops.linear(cV, Lw.linQ_w, Lw.linQ_b, cQ, stream=st)
-            if ref:
-                ops.eltwise(ops.EW_ADD, cV, pl.id_emb[r], tmp, stream=st)
-                ops.linear(tmp, Lw.linV_w, Lw.linV_b, stV, stream=st)
-                ops.eltwise(ops.EW_COPY, cQ, None, stK, stream=st)
-                ops.tc_pack_rows(stK, pl.saKp, 0, stream=st)
-                ops.tc_pack_rows(stV, pl.saVp, 0, stream=st)
-                self._attention(cQ, pl.saKp, pl.saVp, N, n, N, None, core[:, :C], sa_splits, st)
-            else:
-                MN = self.long_term_mem_max * N
-                self._attention(cQ, pl.bank_Kp[li], pl.bank_Vp[li], MN, n, 0, pl.tk[b:b + n], core[:, :C], splits, st)
-            ops.local_attention_tc_batched(cQ, stK, stV, Lw.relk_w, Lw.relk_b, Lw.relv_t, core[:, C:], h, w, H, n, stream=st)
-            ops.linear(core, Lw.lst_proj_w, Lw.lst_proj_b, x, res=x, stream=st)
-            ops.layernorm(x, Lw.norm3[0], Lw.norm3[1], ln, stream=st)
-            ops.linear(ln, Lw.lin1_w, Lw.lin1_b, ff, stream=st)
-            ops.groupnorm(ff.view(n, N, 4 * C), Lw.gn[0], Lw.gn[1], ff.view(n, N, 4 * C), 32, E.A_GELU, pl.gn_ws, stream=st)
-            ops.dwconv(ff.view(n, h, w, 4 * C), Lw.dw_w, None, ff2.view(n, h, w, 4 * C), K=5, pad=2, stream=st)
-            ops.linear(ff2, Lw.lin2_w, Lw.lin2_b, x, res=x, stream=st)
-            ops.layernorm(x, Lw.dec_norm[0], Lw.dec_norm[1], cat[:, (li + 1) * C:(li + 2) * C], stream=st)
+    def _rows(self, b, n):
+        """The LSTT workspace of slots [b, b + n): every activation (and per-layer list) sliced to their rows."""
+        r = slice(b * self._N, (b + n) * self._N)
+        a = types.SimpleNamespace(gn_ws=self._pool.gn_ws)
+        for k, t in self._pool.lstt.items():
+            setattr(a, k, t[r] if isinstance(t, torch.Tensor) else [u[r] for u in t])
+        return a
 
-    def _fuse(self, b, n, st):
-        """AOTEngine._fuse_memories over slots [b, b + n): K = curr_K, V = linear_V(curr_V + id)."""
+    def _lstt(self, b, n, proj, st, ref, splits=None):
+        """engine.aot_lstt over slots [b, b + n): ref = the reference-frame form, else the propagation form over the
+        slots' banks.  Each attention step packs its operands and runs the batched tensor-core kernel."""
         P, pl, N = self._P, self._pool, self._N
-        r = slice(b * N, (b + n) * N)
-        for li in range(P.L):
+        a = self._rows(b, n)
+        sa_splits = E.lt_splits(n * N, P.H, N)
+
+        def own(Q, K, V, out, st, long_term):
+            ops.tc_pack_rows(K, pl.saKp, 0, stream=st)
+            ops.tc_pack_rows(V, pl.saVp, 0, stream=st)
+            self._attention(Q, pl.saKp, pl.saVp, N, n, N, None, out, sa_splits, st)
+
+        def bank(li, Q, out, st):
+            MN = self.long_term_mem_max * N
+            self._attention(Q, pl.bank_Kp[li], pl.bank_Vp[li], MN, n, 0, pl.tk[b:b + n], out, splits, st)
+
+        def local(li, Q, K, V, out, st):
             Lw = P.layers[li]
-            ops.eltwise(ops.EW_ADD, pl.curr_V[li][r], pl.id_emb[r], pl.tmp[r], stream=st)
-            ops.linear(pl.tmp[r], Lw.linV_w, Lw.linV_b, pl.st_V[li][r], stream=st)
-            ops.eltwise(ops.EW_COPY, pl.curr_Q[li][r], None, pl.st_K[li][r], stream=st)
+            ops.local_attention_tc_batched(Q, K, V, Lw.relk_w, Lw.relk_b, Lw.relv_t, out, *self._hw, P.H, n, stream=st)
+
+        E.aot_lstt(P, a, proj, pl.pos[:n * N], self._hw, n, a.st_K, a.st_V, a.id_emb if ref else None, own, bank, local,
+                   st)
 
     def _store(self, b, n, st, flags=None):
         """Store slots [b, b + n)'s short-term K / V into their banks where the store flag is set (flags: written here
@@ -440,39 +404,9 @@ class MultiVideoInferEngine:
                                         pl.flags[b:b + n], n, MN, stream=st)
         ops.ring_advance_batched(pl.tk[b:b + n], pl.wr[b:b + n], pl.flags[b:b + n], n, N, MN, N, stream=st)
 
-    def _dbuf(self, key, shape):
-        t = self._pool.dec.get((key, shape))
-        if t is None:
-            t = self._pool.dec[(key, shape)] = torch.empty(shape, dtype=torch.float32, device=self._pool.x.device)
-        return t
-
     def _decode(self, n):
-        """AOTEngine._decode over the n open videos (B = n) -> their logits [n, h/4, w/4, 11] (NHWC)."""
-        P, pl = self._P, self._pool
-        D = P.dec
-        ac = P.align_corners
-        st = E._cur_stream()
+        """engine.fpn_decode over the n open videos (B = n) -> their logits [n, h/4, w/4, 11] (NHWC)."""
+        pl = self._pool
         x4, x8, x16 = (t[:n] for t in pl.dec_in)
-        h, w = self._hw
-        gws = pl.gn_ws
-
-        def conv_gn(x, blk, key, k, pad):
-            o = self._dbuf(key, (n, x.shape[1], x.shape[2], blk.cout))
-            ops.conv2d(x, blk.w, blk.b, o, KH=k, KW=k, pad=pad, stream=st)
-            ov = o.view(n, -1, blk.cout)
-            ops.groupnorm(ov, blk.gn[0], blk.gn[1], ov, 8, E.A_RELU, gws, stream=st)
-            return o
-
-        x = conv_gn(pl.cat[:n * self._N].view(n, h, w, -1), D.conv_in, "in", 1, 0)
-        a = self._dbuf("a16", (n, h, w, D.adapter_16x.cout))
-        ops.conv2d(x16, D.adapter_16x.w, D.adapter_16x.b, a, res=x, stream=st)
-        x = conv_gn(a, D.conv_16x, "c16", 3, 1)
-        for xs, tag, ad, cv in ((x8, "8", D.adapter_8x, D.conv_8x), (x4, "4", D.adapter_4x, D.conv_4x)):
-            up = self._dbuf("up" + tag, (n, xs.shape[1], xs.shape[2], x.shape[3]))
-            ops.bilinear(x, up, ac, stream=st)
-            a = self._dbuf("a" + tag, (n, xs.shape[1], xs.shape[2], ad.cout))
-            ops.conv2d(xs, ad.w, ad.b, a, res=up, stream=st)
-            x = conv_gn(a, cv, "c" + tag, 3, 1)
-        lg = self._dbuf("logit", (n, x.shape[1], x.shape[2], D.conv_out.cout))
-        ops.conv2d(x, D.conv_out.w, D.conv_out.b, lg, stream=st)
-        return lg
+        return E.fpn_decode(self._P, pl.cat[:n * self._N].view(n, *self._hw, -1), x4, x8, x16, pl.dec, pl.gn_ws,
+                            E._cur_stream())
