@@ -10,11 +10,8 @@ the magnitude of tap j's score, and F_j = sum_c |q_c| / T + |k_c| + |q_c| + |w_c
 
 with u_j = v_j + relv_j (v zero outside the frame): a score error ds moves p by 2 ds relative; the P and V splits cost 2^-21
 relative and the P floor 2^-25 per tap; the fp32 sums over taps and channels add the 2^-23 terms."""
-import math
-
 import pytest
 import torch
-import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
@@ -42,28 +39,8 @@ def _inputs(h, w, qscale, seed):
 
 def _reference(q, k, v, rkw, rkb, rv):
     """float64 oracle output [hw, H*D] and the bound above, both computed on the GPU."""
-    from oracle import aot_oracle as O
-    d = _dev()
-    h, w = q.shape[2], q.shape[3]
-    T = math.sqrt(D)
-    q64, k64, v64, w64, b64, rv64 = (t.to(d, torch.float64) for t in (q, k, v, rkw, rkb, rv))
-    out = O.local_attention(q64, k64, v64, w64, b64, rv64, H)[:, 0]
-    n = h * w
-    rel = F.conv2d(q64, w64, b64, groups=H).view(H, P, n)
-    relmag = F.conv2d(q64.abs(), w64.abs(), b64.abs(), groups=H).view(H, P, n)
-    relfl = F.conv2d(q64.abs(), torch.ones_like(w64), None, groups=H).view(H, P, n) + w64.abs().sum((1, 2, 3)).view(H, P, 1)
-    ku = F.unfold(k64, 15, padding=7).view(H, D, P, n)
-    qv = (q64 / T).view(H, D, n)
-    s = torch.einsum("hdn,hdpn->hpn", qv, ku) + rel
-    inside = F.unfold(torch.ones(1, 1, h, w, dtype=torch.float64, device=d), 15, padding=7).view(1, P, n)
-    p = torch.softmax(s - (1 - inside) * 1e8, dim=1)
-    S = torch.einsum("hdn,hdpn->hpn", qv.abs(), ku.abs()) + relmag
-    Fl = qv.abs().sum(1, keepdim=True) + ku.abs().sum(1) + relfl
-    ds = ((2 ** -21 + U * (8 + 4 * math.sqrt(D))) * S + 2 ** -25 * Fl).amax(1)                  # [H, n]
-    vu = F.unfold(v64.abs(), 15, padding=7).view(H, D, P, n) + rv64.abs().unsqueeze(-1)          # |u_j| per channel
-    pu = torch.einsum("hpn,hdpn->hdn", p, vu)
-    tol = (2 * ds.unsqueeze(1) + 2 ** -21 + U * (8 + 2 * math.sqrt(P))) * pu + 2 ** -25 * vu.sum(2)
-    return out, tol.permute(2, 0, 1).reshape(n, H * D)
+    from test_gpu_local_attn_tc_range import local_law
+    return local_law(q, k, v, rkw, rkb, rv, _dev())
 
 
 def _tok(t):
