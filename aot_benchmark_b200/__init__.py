@@ -6,6 +6,7 @@ Public surface (mirrors the reference's seam, SURVEY 8b):
     EngineConfig(exp, model)              configs/default.py:5-9
     TTAInferEngine(aot_model, ...)        networks/managers/evaluator.py:265-446 with TEST_FLIP / TEST_MULTISCALE
     MultiVideoInferEngine(aot_model, ...) several independent videos propagated in one batched pass per frame
+    DeAOTMultiVideoInferEngine(...)       the same for the DeAOT models
 """
 from .configs import EngineConfig  # noqa: F401
 from .model import build_vos_model  # noqa: F401
@@ -20,7 +21,7 @@ def __getattr__(name):
     if name == "TTAInferEngine":          # imported on first use, like the engines behind build_engine
         from .tta import TTAInferEngine
         return TTAInferEngine
-    if name == "MultiVideoInferEngine":
-        from .multi_video import MultiVideoInferEngine
-        return MultiVideoInferEngine
+    if name in ("MultiVideoInferEngine", "DeAOTMultiVideoInferEngine"):
+        from . import multi_video
+        return getattr(multi_video, name)
     raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

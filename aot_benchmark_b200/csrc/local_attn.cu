@@ -703,8 +703,10 @@ static int launch_local_tc(const LocalArgs& a, const float* relv_t, cudaStream_t
 // The generic per-warp kernel (local_attn_kernel<128, 1024>) re-reads K / V rows from L1 / L2 for every query: 226 us per launch
 // at 31 x 54 (19.6 % of the R50-DeAOTL frame).  Here a CTA re-computes the scores of its query tile for its channel group
 // (VC = 8: 4 groups of 256 channels -> 144 CTAs, one wave) and reads every halo row once per chunk.
+// One CTA of the tiled DeAOT local attention over the map whose q / k / v / out rows `p` points at (taken by value: passed by
+// reference, the one-map kernel schedules differently).
 template <int TY, int TX, int KC, int VC>
-__global__ void __launch_bounds__(512, 1) local_gated_tile_kernel(const LocalArgs p) {
+__device__ __forceinline__ void local_gated_tile_cta(const LocalArgs p) {
     pdl_sync();
     constexpr int C = 32, HH = TY + 2 * LR, HWD = TX + 2 * LR, NPOS = HH * HWD, LD = 36;
     constexpr int NT = 512, NQ = TY * TX, PLD = LW * 16, DQ = KC * C;
@@ -885,22 +887,45 @@ __global__ void __launch_bounds__(512, 1) local_gated_tile_kernel(const LocalArg
     }
 }
 
-static int launch_local_gated_tile(const LocalArgs& a, cudaStream_t st) {
-    constexpr int TY = 8, TX = 6, KC = 4, VC = 8;       // d_att = 128; 1024 value channels = 4 groups of 8 chunks
-    const size_t smem = sizeof(float) * (size_t)((TY + 14) * (TX + 14) * 36 + TY * TX * KC * 32 + TY * TX * LW * 16);
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(local_gated_tile_kernel<TY, TX, KC, VC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)smem);
+template <int TY, int TX, int KC, int VC>
+__global__ void __launch_bounds__(512, 1) local_gated_tile_kernel(const LocalArgs p) {
+    local_gated_tile_cta<TY, TX, KC, VC>(p);
+}
+
+// n maps of h x w pixels stacked along the rows: map b = blockIdx.z is rows [b h w, (b + 1) h w) of q, k, v and out.
+template <int TY, int TX, int KC, int VC>
+__global__ void __launch_bounds__(512, 1) local_gated_tile_batched_kernel(const LocalArgs p) {
+    const size_t r0 = (size_t)blockIdx.z * p.h * p.w;
+    LocalArgs pb = p;
+    pb.q += r0 * p.ldq;
+    pb.k += r0 * p.ldk;
+    pb.v += r0 * p.ldv;
+    pb.out += r0 * p.ldo;
+    local_gated_tile_cta<TY, TX, KC, VC>(pb);
+}
+
+// the tiling of the DeAOT tile kernels: d_att = 128 in KC = 4 chunks; 1024 value channels = 4 groups of VC = 8 chunks
+constexpr int LGT_TY = 8, LGT_TX = 6, LGT_KC = 4, LGT_VC = 8;
+constexpr size_t LGT_SMEM = sizeof(float) * (size_t)((LGT_TY + 14) * (LGT_TX + 14) * 36 + LGT_TY * LGT_TX * LGT_KC * 32 +
+                                                     LGT_TY * LGT_TX * LW * 16);
+
+// n = 0: the one-map kernel; n >= 1: the batched kernel over n maps
+static int launch_local_gated_tile(const LocalArgs& a, int n, cudaStream_t st) {
+    auto k1 = local_gated_tile_kernel<LGT_TY, LGT_TX, LGT_KC, LGT_VC>;
+    auto kn = local_gated_tile_batched_kernel<LGT_TY, LGT_TX, LGT_KC, LGT_VC>;
+    const char* what = n ? "aotb_local_gated_tile_batched_f32" : "aotb_local_gated_tile_f32";
+    static bool configured[2] = {false, false};
+    if (!configured[n ? 1 : 0]) {
+        cudaError_t e = cudaFuncSetAttribute(n ? kn : k1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LGT_SMEM);
         if (e != cudaSuccess) {
-            set_error("aotb_local_gated_tile_f32: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+            set_error("%s: cudaFuncSetAttribute: %s", what, cudaGetErrorString(e));
             return AOTB_ERR_CUDA;
         }
-        configured = true;
+        configured[n ? 1 : 0] = true;
     }
-    dim3 grid(cdiv(a.h, TY) * cdiv(a.w, TX), 1024 / (VC * 32));
-    launch(local_gated_tile_kernel<TY, TX, KC, VC>, dim3(grid), dim3(512), smem, st, a);
-    return check_launch("aotb_local_gated_tile_f32");
+    dim3 grid(cdiv(a.h, LGT_TY) * cdiv(a.w, LGT_TX), 1024 / (LGT_VC * 32), n ? n : 1);
+    launch(n ? kn : k1, grid, dim3(512), LGT_SMEM, st, a);
+    return check_launch(what);
 }
 
 }  // namespace aotb
@@ -964,7 +989,7 @@ extern "C" int aotb_local_gated_tile_f32(const float* q, int ldq, const float* k
     a.q = q; a.ldq = ldq; a.k = k; a.ldk = ldk; a.v = v; a.ldv = ldv;
     a.relk_w = relk_w; a.relk_b = relk_b; a.relv = nullptr; a.out = out; a.ldo = ldo;
     a.h = h; a.w = w; a.H = 1; a.T = sqrtf(128.f);
-    return launch_local_gated_tile(a, (cudaStream_t)stream);
+    return launch_local_gated_tile(a, 0, (cudaStream_t)stream);
 }
 
 // n maps of h x w pixels stacked along the rows of q, k, v and out (map b = rows [b h w, (b + 1) h w)); map b's output is bit
@@ -982,4 +1007,19 @@ extern "C" int aotb_local_attention_tc_batched_f32(const float* q, int ldq, cons
     a.relk_w = relk_w; a.relk_b = relk_b; a.relv = nullptr; a.out = out; a.ldo = ldo;
     a.h = h; a.w = w; a.H = H; a.T = sqrtf(32.f);
     return launch_local_tc_batched(a, relv_t, n, (cudaStream_t)stream);
+}
+
+// n maps of h x w pixels stacked along the rows of q, k, v and out (map b = rows [b h w, (b + 1) h w)); map b's output is bit
+// for bit aotb_local_gated_tile_f32 on its rows.
+extern "C" int aotb_local_gated_tile_batched_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                                                 const float* relk_w, const float* relk_b, float* out, int ldo, int h, int w,
+                                                 int n, void* stream) {
+    AOTB_REQUIRE(q && k && v && relk_w && relk_b && out && h > 0 && w > 0 && n >= 1 && n <= 65535,
+                 "aotb_local_gated_tile_batched_f32: bad args");
+    AOTB_REQUIRE(ldq % 4 == 0 && ldk % 4 == 0 && ldv % 4 == 0, "aotb_local_gated_tile_batched_f32: ld %% 4");
+    LocalArgs a;
+    a.q = q; a.ldq = ldq; a.k = k; a.ldk = ldk; a.v = v; a.ldv = ldv;
+    a.relk_w = relk_w; a.relk_b = relk_b; a.relv = nullptr; a.out = out; a.ldo = ldo;
+    a.h = h; a.w = w; a.H = 1; a.T = sqrtf(128.f);
+    return launch_local_gated_tile(a, n, (cudaStream_t)stream);
 }

@@ -732,6 +732,119 @@ def fpn_decode(P, cat_nhwc, x4, x8, x16, dbuf, gn_ws, st):
     return lg
 
 
+# DeAOT: the gated propagation module stack (transformer.py:501-665) over n maps, shared by DeAOTEngine and
+# DeAOTMultiVideoInferEngine as aot_lstt is by the AOT engines
+def gp_splits(n_queries, C, Tk):
+    """KV-split count of the fused DeAOT long-term attention kernel over n_queries query rows (one CTA = 128 queries x 64
+    value channels x one split): about two waves of CTAs, at least four 64-key tiles per split."""
+    base = ((n_queries + 127) // 128) * (4 * C // 64)
+    tiles = (max(Tk, 1) + 63) // 64
+    return max(1, min(tiles // 4 if tiles >= 8 else 1, max(1, (2 * 132) // base)))
+
+
+def _deaot_gpm_buffers(rows, C, L, device):
+    """DeAOT's fp32 activations over `rows` token rows, by name (curr_Q, curr_V, curr_IDV, st_K, st_V: per-layer lists;
+    curr_IDV[0] is None, layer 0 has no ID stream input), in the one-video engine's allocation order."""
+    f = lambda c: torch.empty((rows, c), dtype=torch.float32, device=device)
+    d = C // 2
+    out = {k: f(m) for k, m in (("id_emb", C), ("xz", 2 * C), ("ln", C), ("qv", d + 2 * C), ("catU", 4 * C),
+                                ("idin", 2 * C), ("core", 4 * C), ("gated", 4 * C), ("dw", 8 * C), ("c", 2 * C),
+                                ("sa_qk", d), ("sa_v", 4 * C), ("sa_u", 4 * C), ("cat", 2 * C))}
+    out["curr_Q"] = [f(d) for _ in range(L)]
+    out["curr_V"] = [f(2 * C) for _ in range(L)]
+    out["curr_IDV"] = [None] + [f(C) for _ in range(L - 1)]
+    out["st_K"] = [f(d) for _ in range(L)]
+    out["st_V"] = [f(4 * C) for _ in range(L)]   # cat[V | ID_V] (transformer.py:625-626)
+    return out
+
+
+def _gated_tail(a, core, U, dw_w, out, n, hw, st):
+    """(attn @ V) * U -> depthwise 5x5 (attention.py:707-709 / :855-857) over n maps; the projection is fused later."""
+    h, w = hw
+    C4 = core.shape[1]
+    ops.eltwise(ops.EW_MUL, core, U, a.gated, stream=st)
+    ops.dwconv(a.gated.view(n, h, w, C4), dw_w, None, out.unflatten(0, (n, h, w)), K=5, pad=2, stream=st)
+
+
+def _deaot_fuse_id(Lw, a, C, cIDV, id_emb, out, st):
+    """GatedPropagationModule.fuse_key_value_id (transformer.py:659-665) of one layer."""
+    if cIDV is None:
+        ops.linear(id_emb, Lw.idv_w, Lw.idv_b, out, act=A_SILU, stream=st)
+    else:
+        ops.eltwise(ops.EW_COPY, cIDV, None, a.idin[:, :C], stream=st)
+        ops.eltwise(ops.EW_COPY, id_emb, None, a.idin[:, C:], stream=st)
+        ops.linear(a.idin, Lw.idv_w, Lw.idv_b, out, act=A_SILU, stream=st)
+
+
+def deaot_fuse_memories(P, a, id_emb, K, V, st):
+    """deaot_engine.py:20-45 over the rows of workspace `a`: the short-term K[li] = curr_Q and V[li] = [curr_V | ID_V] of
+    every layer, ID_V = fuse_key_value_id(curr_ID_V, id_emb)."""
+    C2 = 2 * P.C
+    for li in range(P.L):
+        ops.eltwise(ops.EW_COPY, a.curr_Q[li], None, K[li], stream=st)
+        ops.eltwise(ops.EW_COPY, a.curr_V[li], None, V[li][:, :C2], stream=st)
+        _deaot_fuse_id(P.layers[li], a, P.C, a.curr_IDV[li], id_emb, V[li][:, C2:], st)
+
+
+def deaot_lstt(P, a, proj, hw, n, st_K, st_V, id_emb, attend_own, attend_bank, local, st):
+    """The DeAOT LSTT (GatedPropagationModule stack, transformer.py:590-665, and its final GroupNorm, :197-200) over n maps of
+    hw = (h, w) tokens stacked in the rows of workspace `a` (the activations of _deaot_gpm_buffers sliced to those rows, and
+    the groupnorm workspace gn_ws for n maps); proj: their projected 16x features.  id_emb None: a propagated frame, whose
+    long-term step reads the bank; else a reference frame, whose short-term K / V (st_K, st_V) are fused first and are its
+    long-term memory.  The engine's hooks launch the attention steps:
+      attend_own(Q, K, V, out, st, long_term)   over the frame's own K / V: the gated self-attention, and (long_term=True)
+                                                the reference frame's long-term step
+      attend_bank(li, Q, out, st)               the long-term step over layer li's bank
+      local(li, Q, K, V, out, st)               the short-term gated local attention"""
+    C = P.C
+    h, w = hw
+    d, C2, C4 = C // 2, 2 * C, 4 * C
+    x, z = a.xz[:, :C], a.xz[:, C:]
+    ops.eltwise(ops.EW_COPY, proj, None, x, stream=st)
+    ops.eltwise(ops.EW_FILL, None, None, z, scalar=0.0, stream=st)        # tgt_id = 0 (transformer.py:603)
+    for li in range(P.L):
+        Lw = P.layers[li]
+        cQ, cV = a.curr_Q[li], a.curr_V[li]
+        ops.layernorm(x, Lw.norm1[0], Lw.norm1[1], a.ln, stream=st)
+        ops.linear(a.ln, Lw.qv_w, Lw.qv_b, a.qv, stream=st)
+        ops.eltwise(ops.EW_COPY, a.qv[:, :d], None, cQ, stream=st)
+        ops.eltwise(ops.EW_SILU, a.qv[:, d:], None, cV, stream=st)          # curr_V = silu(.) :599
+        ops.linear(a.ln, Lw.u_w, Lw.u_b, a.catU[:, :C2], act=A_SILU, stream=st)
+        if li == 0:
+            ops.eltwise(ops.EW_FILL, None, None, a.catU[:, C2:], scalar=1.0, stream=st)   # :604-605
+            cIDV = None
+        else:
+            cIDV = a.curr_IDV[li]
+            ops.layernorm(z, Lw.id_norm1[0], Lw.id_norm1[1], cIDV, stream=st)
+            ops.linear(cIDV, Lw.idu_w, Lw.idu_b, a.catU[:, C2:], act=A_SILU, stream=st)    # :610-611
+        if id_emb is not None:
+            ops.eltwise(ops.EW_COPY, cQ, None, st_K[li], stream=st)
+            ops.eltwise(ops.EW_COPY, cV, None, st_V[li][:, :C2], stream=st)
+            _deaot_fuse_id(Lw, a, C, cIDV, id_emb, st_V[li][:, C2:], st)
+            attend_own(cQ, st_K[li], st_V[li], a.core, st, True)
+        else:
+            attend_bank(li, cQ, a.core, st)
+        _gated_tail(a, a.core, a.catU, Lw.lt_dw, a.dw[:, :C4], n, hw, st)
+        local(li, cQ, st_K[li], st_V[li], a.core, st)
+        _gated_tail(a, a.core, a.catU, Lw.st_dw, a.dw[:, C4:], n, hw, st)
+        # [tgt | tgt_id] += proj_lt(.) + proj_st(.)   (transformer.py:633-641) as one K = 8C GEMM
+        ops.linear(a.dw, Lw.lst_proj_w, Lw.lst_proj_b, a.xz, res=a.xz, stream=st)
+        # gated self-attention on both streams (transformer.py:644-653, attention.py:648-669)
+        ops.layernorm(x, Lw.norm2[0], Lw.norm2[1], a.c[:, :C], stream=st)
+        ops.layernorm(z, Lw.id_norm2[0], Lw.id_norm2[1], a.c[:, C:], stream=st)
+        ops.linear(a.c, Lw.sa_qk_w, Lw.sa_qk_b, a.sa_qk, stream=st)
+        ops.linear(a.c[:, :C], Lw.sa_v1[0], Lw.sa_v1[1], a.sa_v[:, :C2], act=A_SILU, stream=st)
+        ops.linear(a.c[:, C:], Lw.sa_v2[0], Lw.sa_v2[1], a.sa_v[:, C2:], act=A_SILU, stream=st)
+        ops.linear(a.c[:, :C], Lw.sa_u1[0], Lw.sa_u1[1], a.sa_u[:, :C2], act=A_SILU, stream=st)
+        ops.linear(a.c[:, C:], Lw.sa_u2[0], Lw.sa_u2[1], a.sa_u[:, C2:], act=A_SILU, stream=st)
+        attend_own(a.sa_qk, a.sa_qk, a.sa_v, a.core, st, False)
+        _gated_tail(a, a.core, a.sa_u, Lw.sa_dw, a.dw[:, :C4], n, hw, st)
+        ops.linear(a.dw[:, :C4], Lw.sa_proj_w, Lw.sa_proj_b, a.xz, res=a.xz, stream=st)
+    # final GroupNorm1D(2C, groups=2) (transformer.py:197-200,241) -> decoder input
+    ops.groupnorm(a.xz.view(n, h * w, C2), P.final_gn[0], P.final_gn[1], a.cat.view(n, h * w, C2), 2, A_NONE, a.gn_ws,
+                  stream=st)
+
+
 # =====================================================================================
 # single engine (<= max_obj_num objects)
 # =====================================================================================
@@ -879,27 +992,11 @@ class AOTEngine(nn.Module):
             self.curr_Q, self.curr_V = ws.curr_Q, ws.curr_V
             self._kdim, self._vdim = C, C
         else:
-            d = C // 2
-            ws.id_emb = f(N, C)
-            ws.xz = f(N, 2 * C)
-            ws.ln = f(N, C)
-            ws.qv = f(N, d + 2 * C)
-            ws.catU = f(N, 4 * C)
-            ws.idin = f(N, 2 * C)
-            ws.core = f(N, 4 * C)
-            ws.gated = f(N, 4 * C)
-            ws.dw = f(N, 8 * C)
-            ws.c = f(N, 2 * C)
-            ws.sa_qk = f(N, d)
-            ws.sa_v = f(N, 4 * C)
-            ws.sa_u = f(N, 4 * C)
-            ws.cat = f(N, 2 * C)
-            self.curr_Q = [f(N, d) for _ in range(L)]
-            self.curr_V = [f(N, 2 * C) for _ in range(L)]
-            self.curr_IDV = [None] + [f(N, C) for _ in range(L - 1)]
-            self.st_K = [f(N, d) for _ in range(L)]
-            self.st_V = [f(N, 4 * C) for _ in range(L)]   # cat[V | ID_V] (transformer.py:625-626)
-            self._kdim, self._vdim = d, 4 * C
+            bufs = _deaot_gpm_buffers(N, C, L, dev)
+            self.st_K, self.st_V = bufs.pop("st_K"), bufs.pop("st_V")     # the live slot: _commit_short_slot moves it
+            vars(ws).update(bufs)
+            self.curr_Q, self.curr_V, self.curr_IDV = ws.curr_Q, ws.curr_V, ws.curr_IDV
+            self._kdim, self._vdim = C // 2, 4 * C
         ws.mask = f(*self.input_size_2d)                            # static copy of the caller's label map
         self._dec_out = {}
         cap = (min(BANK_INIT_FRAMES, GEMM_GROW_FRAMES) if (P.deaot and DEAOT_LT == "gemm") else BANK_INIT_FRAMES) * N
@@ -1571,102 +1668,56 @@ class DeAOTEngine(AOTEngine):
                          precision=precision, long_term_mem_policy=long_term_mem_policy)
         self.layer_loss_scaling_ratio = layer_loss_scaling_ratio
 
-    def _gated_tail(self, core, U, dw_w, out_slice, h, w, st):
-        """(attn @ V) * U -> depthwise 5x5 (attention.py:707-709 / :855-857); projection is fused later."""
-        ws = self._ws
-        N = core.shape[0]
-        C4 = core.shape[1]
-        ops.eltwise(ops.EW_MUL, core, U, ws.gated, stream=st)
-        ops.dwconv(ws.gated.view(1, h, w, C4), dw_w, None, out_slice.unflatten(0, (1, h, w)), K=5, pad=2, stream=st)
-
     def _lstt_forward(self, embs, id_emb, st):
         P = self._plan()
-        ws = self._ws
-        N, C = self.enc_hw, P.C
-        h, w = self.enc_size_2d
-        d = C // 2
-        C2, C4 = 2 * C, 4 * C
-        proj = embs.nhwc[-1].view(N, C)
-        x, z = ws.xz[:, :C], ws.xz[:, C:]
-        ops.eltwise(ops.EW_COPY, proj, None, x, stream=st)
-        ops.eltwise(ops.EW_FILL, None, None, z, scalar=0.0, stream=st)        # tgt_id = 0 (transformer.py:603)
-        is_ref = id_emb is not None
-        if is_ref:
-            stK, stV = self._next_short_slot()
-        else:
-            stK, stV = self.st_K, self.st_V
-        for li in range(P.L):
-            Lw = P.layers[li]
-            cQ, cV = self.curr_Q[li], self.curr_V[li]
-            ops.layernorm(x, Lw.norm1[0], Lw.norm1[1], ws.ln, stream=st)
-            ops.linear(ws.ln, Lw.qv_w, Lw.qv_b, ws.qv, stream=st)
-            ops.eltwise(ops.EW_COPY, ws.qv[:, :d], None, cQ, stream=st)
-            ops.eltwise(ops.EW_SILU, ws.qv[:, d:], None, cV, stream=st)          # curr_V = silu(.) :599
-            ops.linear(ws.ln, Lw.u_w, Lw.u_b, ws.catU[:, :C2], act=A_SILU, stream=st)
-            if li == 0:
-                ops.eltwise(ops.EW_FILL, None, None, ws.catU[:, C2:], scalar=1.0, stream=st)   # :604-605
-                cIDV = None
-            else:
-                cIDV = self.curr_IDV[li]
-                ops.layernorm(z, Lw.id_norm1[0], Lw.id_norm1[1], cIDV, stream=st)
-                ops.linear(cIDV, Lw.idu_w, Lw.idu_b, ws.catU[:, C2:], act=A_SILU, stream=st)    # :610-611
-            if is_ref:
-                ops.eltwise(ops.EW_COPY, cQ, None, stK[li], stream=st)
-                ops.eltwise(ops.EW_COPY, cV, None, stV[li][:, :C2], stream=st)
-                self._fuse_id(li, cIDV, id_emb, stV[li][:, C2:], st)
-                gK, gV, Tk = stK[li], stV[li], N
-            else:
-                gK, gV, Tk = self.bank_K[li], self.bank_V[li], self.bank_len
-            probe = LT_PROBE if not is_ref else None
-            if probe is not None:
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-            if self._gp_tc and not is_ref and self._usage():
-                ops.tc_pack_rows(cQ, ws.gpQp, 0, div=math.sqrt(self._kdim), stream=st)
-                self._usage_attention(li, ws.gpQp, self.bank_gpK[li], self.bank_gpV[li], ws.core, st)
-            elif self._gp_tc and not is_ref:
-                # fused wgmma kernel (gp_attn_tc.cu): 128 queries x 64 value channels per CTA, KV splits to fill the GPU
-                self._gp_attention(cQ, None, None, self.bank_gpK[li], self.bank_gpV[li], Tk, self.tk_dev, ws.core, st)
-            elif self._gp_tc:
-                self._gp_attention(cQ, gK, gV, None, None, N, None, ws.core, st)     # reference frame: its own K / V
-            elif self._gemm_lt and not is_ref:
-                # S = Q K^T -> softmax(S / T) over the live keys -> P V, all on the tensor-core GEMM (deaot_lt.cu)
-                ops.linear_tc(cQ, self.bank_Kh[li], self.bank_Kl[li], None, ws.S, stream=st)
-                ops.row_softmax(ws.S, self._capw, Tk, 1.0 / math.sqrt(d), Tk_dev=self.tk_dev, stream=st)
-                ops.linear_tc(ws.S, self.bank_VhT[li], self.bank_VlT[li], None, ws.core, stream=st)
-            else:
-                ops.attention(cQ, gK, gV, ws.core, 1, d, C4, Tk=Tk, Tk_dev=None if is_ref else self.tk_dev, stream=st)
-            if probe is not None:
-                e1.record()
-                probe.append((e0, e1, 2.0 * N * Tk * (d + C4)))      # FLOPs = 2*N*Tk*(d_qk + d_v), SURVEY 8d
-            self._gated_tail(ws.core, ws.catU, Lw.lt_dw, ws.dw[:, :C4], h, w, st)
-            if LOCAL_IMPL != "warp" and d == 128 and C4 == 1024:
-                ops.local_gated_tile(cQ, stK[li], stV[li], Lw.relk_w, Lw.relk_b, ws.core, h, w, stream=st)
-            else:
-                ops.local_attention(cQ, stK[li], stV[li], Lw.relk_w, Lw.relk_b, None, ws.core, h, w, 1, d, C4, stream=st)
-            self._gated_tail(ws.core, ws.catU, Lw.st_dw, ws.dw[:, C4:], h, w, st)
-            # [tgt | tgt_id] += proj_lt(.) + proj_st(.)   (transformer.py:633-641) as one K = 8C GEMM
-            ops.linear(ws.dw, Lw.lst_proj_w, Lw.lst_proj_b, ws.xz, res=ws.xz, stream=st)
-            # gated self-attention on both streams (transformer.py:644-653, attention.py:648-669)
-            ops.layernorm(x, Lw.norm2[0], Lw.norm2[1], ws.c[:, :C], stream=st)
-            ops.layernorm(z, Lw.id_norm2[0], Lw.id_norm2[1], ws.c[:, C:], stream=st)
-            ops.linear(ws.c, Lw.sa_qk_w, Lw.sa_qk_b, ws.sa_qk, stream=st)
-            ops.linear(ws.c[:, :C], Lw.sa_v1[0], Lw.sa_v1[1], ws.sa_v[:, :C2], act=A_SILU, stream=st)
-            ops.linear(ws.c[:, C:], Lw.sa_v2[0], Lw.sa_v2[1], ws.sa_v[:, C2:], act=A_SILU, stream=st)
-            ops.linear(ws.c[:, :C], Lw.sa_u1[0], Lw.sa_u1[1], ws.sa_u[:, :C2], act=A_SILU, stream=st)
-            ops.linear(ws.c[:, C:], Lw.sa_u2[0], Lw.sa_u2[1], ws.sa_u[:, C2:], act=A_SILU, stream=st)
-            if self._gp_tc:
-                self._gp_attention(ws.sa_qk, ws.sa_qk, ws.sa_v, None, None, N, None, ws.core, st)
-            else:
-                ops.attention(ws.sa_qk, ws.sa_qk, ws.sa_v, ws.core, 1, d, C4, Tk=N, stream=st)
-            self._gated_tail(ws.core, ws.sa_u, Lw.sa_dw, ws.dw[:, :C4], h, w, st)
-            ops.linear(ws.dw[:, :C4], Lw.sa_proj_w, Lw.sa_proj_b, ws.xz, res=ws.xz, stream=st)
-        # final GroupNorm1D(2C, groups=2) (transformer.py:197-200,241) -> decoder input
-        ops.groupnorm(ws.xz.view(1, N, C2), P.final_gn[0], P.final_gn[1], ws.cat.view(1, N, C2), 2, A_NONE, ws.gn_ws,
-                      stream=st)
-        if is_ref:
+        stK, stV = (self.st_K, self.st_V) if id_emb is None else self._next_short_slot()
+        deaot_lstt(P, self._ws, embs.nhwc[-1].view(self.enc_hw, P.C), self.enc_size_2d, 1, stK, stV, id_emb,
+                   self._attend_own, self._attend_bank, self._local_attention, st)
+        if id_emb is not None:
             self._commit_short_slot(stK, stV)
         self._have_lstt = True
+
+    def _attend_own(self, Q, K, V, out, st, long_term):
+        """softmax(Q K^T / T) V over the frame's own K / V: the gated self-attention, or (long_term) a reference frame's
+        long-term step (transformer.py:614-616)."""
+        if self._gp_tc:
+            self._gp_attention(Q, K, V, None, None, self.enc_hw, None, out, st)
+        else:
+            ops.attention(Q, K, V, out, 1, self._kdim, self._vdim, Tk=self.enc_hw, stream=st)
+
+    def _attend_bank(self, li, Q, out, st):
+        """The long-term step of a propagated frame over layer li's bank, which LT_PROBE times."""
+        ws = self._ws
+        Tk = self.bank_len
+        probe = LT_PROBE
+        if probe is not None:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+        if self._gp_tc and self._usage():
+            ops.tc_pack_rows(Q, ws.gpQp, 0, div=math.sqrt(self._kdim), stream=st)
+            self._usage_attention(li, ws.gpQp, self.bank_gpK[li], self.bank_gpV[li], out, st)
+        elif self._gp_tc:
+            # fused wgmma kernel (gp_attn_tc.cu): 128 queries x 64 value channels per CTA, KV splits to fill the GPU
+            self._gp_attention(Q, None, None, self.bank_gpK[li], self.bank_gpV[li], Tk, self.tk_dev, out, st)
+        elif self._gemm_lt:
+            # S = Q K^T -> softmax(S / T) over the live keys -> P V, all on the tensor-core GEMM (deaot_lt.cu)
+            ops.linear_tc(Q, self.bank_Kh[li], self.bank_Kl[li], None, ws.S, stream=st)
+            ops.row_softmax(ws.S, self._capw, Tk, 1.0 / math.sqrt(self._kdim), Tk_dev=self.tk_dev, stream=st)
+            ops.linear_tc(ws.S, self.bank_VhT[li], self.bank_VlT[li], None, out, stream=st)
+        else:
+            ops.attention(Q, self.bank_K[li], self.bank_V[li], out, 1, self._kdim, self._vdim, Tk=Tk, Tk_dev=self.tk_dev,
+                          stream=st)
+        if probe is not None:
+            e1.record()
+            probe.append((e0, e1, 2.0 * self.enc_hw * Tk * (self._kdim + self._vdim)))   # FLOPs = 2*N*Tk*(d_qk + d_v), SURVEY 8d
+
+    def _local_attention(self, li, Q, K, V, out, st):
+        Lw = self._plan().layers[li]
+        h, w = self.enc_size_2d
+        if LOCAL_IMPL != "warp" and self._kdim == 128 and self._vdim == 1024:
+            ops.local_gated_tile(Q, K, V, Lw.relk_w, Lw.relk_b, out, h, w, stream=st)
+        else:
+            ops.local_attention(Q, K, V, Lw.relk_w, Lw.relk_b, None, out, h, w, 1, self._kdim, self._vdim, stream=st)
 
     def _gp_attention(self, Q, K, V, Kp, Vp, Tk, Tk_dev, out, st):
         """softmax(Q K^T / T) V for the DeAOT head shape (1 x 128 / 1024) on the fused wgmma kernel.  Q fp32 [N, 128] is
@@ -1685,33 +1736,13 @@ class DeAOTEngine(AOTEngine):
                             part=part, stream=st)
 
     def _gp_splits(self, Tk):
-        """KV-split count of the fused DeAOT long-term attention kernel (one CTA = 128 queries x 64 value channels x one
-        split): about two waves of CTAs, at least four 64-key tiles per split."""
-        base = ((self.enc_hw + 127) // 128) * (4 * self._plan().C // 64)
-        tiles = (max(Tk, 1) + 63) // 64
-        return max(1, min(tiles // 4 if tiles >= 8 else 1, max(1, (2 * 132) // base)))
-
-    def _fuse_id(self, li, cIDV, id_emb, out, st):
-        """GatedPropagationModule.fuse_key_value_id (transformer.py:659-665)."""
-        Lw = self._plan().layers[li]
-        ws = self._ws
-        C = self._plan().C
-        if cIDV is None:
-            ops.linear(id_emb, Lw.idv_w, Lw.idv_b, out, act=A_SILU, stream=st)
-        else:
-            ops.eltwise(ops.EW_COPY, cIDV, None, ws.idin[:, :C], stream=st)
-            ops.eltwise(ops.EW_COPY, id_emb, None, ws.idin[:, C:], stream=st)
-            ops.linear(ws.idin, Lw.idv_w, Lw.idv_b, out, act=A_SILU, stream=st)
+        """gp_splits over this engine's query rows."""
+        return gp_splits(self.enc_hw, self._plan().C, Tk)
 
     def _fuse_memories(self, id_emb, st):
         """deaot_engine.py:20-45: K, V unchanged; ID_V = fuse_key_value_id(None, curr_ID_V, id_emb)."""
-        P = self._plan()
-        C2 = 2 * P.C
         K, V = self._next_short_slot()
-        for li in range(P.L):
-            ops.eltwise(ops.EW_COPY, self.curr_Q[li], None, K[li], stream=st)
-            ops.eltwise(ops.EW_COPY, self.curr_V[li], None, V[li][:, :C2], stream=st)
-            self._fuse_id(li, self.curr_IDV[li], id_emb, V[li][:, C2:], st)
+        deaot_fuse_memories(self._plan(), self._ws, id_emb, K, V, st)
         self._commit_short_slot(K, V, reset=False)
 
 

@@ -1,10 +1,10 @@
 """Several independent videos propagated through one engine, one batched encoder + LSTT + decoder pass per frame.
 
-Per video, the semantics are those of AOTInferEngine(long_term_mem_max=M) with at most 10 objects: each video has its own
-frame step, object count, long-term gap, short-term memory and bounded long-term bank (the first memory frame pinned, the
-newest M - 1 in a ring).  Videos open and close independently; the n open videos always occupy slots 0 .. n - 1 of a pool
-allocated once per (geometry, S, M), so every launch covers exactly n videos and every captured graph is keyed on n (DESIGN
-§3.9).
+Per video, the semantics are those of AOTInferEngine(long_term_mem_max=M) with at most 10 objects (DeAOTInferEngine for
+DeAOTMultiVideoInferEngine): each video has its own frame step, object count, long-term gap, short-term memory and bounded
+long-term bank (the first memory frame pinned, the newest M - 1 in a ring).  Videos open and close independently; the n open
+videos always occupy slots 0 .. n - 1 of a pool allocated once per (geometry, S, M), so every launch covers exactly n videos
+and every captured graph is keyed on n (DESIGN §3.9).
 """
 from __future__ import annotations
 
@@ -34,36 +34,23 @@ class MultiVideoInferEngine:
     def __init__(self, aot_model, max_videos=4, long_term_mem_max=None, gpu_id=0, long_term_mem_gap=None,
                  short_term_mem_skip=1, precision=None, long_term_mem_policy=None):
         cfg = aot_model.cfg
-        if cfg.MODEL_VOS == "deaot":
-            raise NotImplementedError("MultiVideoInferEngine runs the AOT models; DeAOT's gated propagation has no batched "
-                                      "entry points yet")
+        self._check_family(cfg)
         policy = getattr(cfg, "TEST_LONG_TERM_MEM_POLICY", None) if long_term_mem_policy is None else long_term_mem_policy
         if policy is not None and policy not in E.MEM_POLICIES:
             raise ValueError(f"long_term_mem_policy must be one of {E.MEM_POLICIES}, got {policy!r}")
+        name = type(self).__name__
         if policy not in (None, "fifo"):
-            raise NotImplementedError("MultiVideoInferEngine keeps FIFO banks; long_term_mem_policy='usage' counts attention "
-                                      "mass per video, which the batched attention does not")
-        if E.LT_IMPL == "simt":
-            raise NotImplementedError("MultiVideoInferEngine runs the tensor-core long-term attention; AOTB_LT_IMPL=simt "
-                                      "selects the fp32 CUDA-core kernel")
-        if ops.CONV_IMPL == "simt":
-            raise NotImplementedError("MultiVideoInferEngine runs the tensor-core conv; AOTB_CONV_IMPL=simt selects the fp32 "
-                                      "CUDA-core conv")
-        if ops.LT_VARIANT != "tile":
-            raise NotImplementedError(f"MultiVideoInferEngine runs the default 'tile' layout of the long-term attention; "
-                                      f"AOTB_LT_VARIANT={ops.LT_VARIANT} selects another")
-        if E.LOCAL_IMPL != "tc":
-            raise NotImplementedError(f"MultiVideoInferEngine runs the tensor-core local attention; AOTB_LOCAL_IMPL="
-                                      f"{E.LOCAL_IMPL} selects a CUDA-core kernel")
+            raise NotImplementedError(f"{name} keeps FIFO banks; long_term_mem_policy='usage' counts attention mass per "
+                                      f"video, which the batched attention does not")
+        self._check_kernels()
         if short_term_mem_skip != 1:
-            raise NotImplementedError("MultiVideoInferEngine keeps one short-term memory frame per video "
-                                      "(short_term_mem_skip=1)")
+            raise NotImplementedError(f"{name} keeps one short-term memory frame per video (short_term_mem_skip=1)")
         if int(max_videos) != max_videos or max_videos < 1:
             raise ValueError(f"max_videos must be a positive integer, got {max_videos}")
         M = E._resolve_mem_max(aot_model, long_term_mem_max)
         if M is None:
-            raise ValueError("MultiVideoInferEngine pools a bounded long-term bank per video: give long_term_mem_max (or "
-                             "cfg.TEST_LONG_TERM_MEM_MAX)")
+            raise ValueError(f"{name} pools a bounded long-term bank per video: give long_term_mem_max (or "
+                             f"cfg.TEST_LONG_TERM_MEM_MAX)")
         self.precision = E._resolve_precision(aot_model, precision)
         self.AOT, self.cfg = aot_model, cfg
         self.max_videos, self.long_term_mem_max = int(max_videos), M
@@ -80,10 +67,33 @@ class MultiVideoInferEngine:
         self._slots = []                 # slot -> per-video host state (dict); slot order = stacking order of every buffer
         self._next_vid = 0
 
+    # per-layer workspace buffers that carry a video's state from propagate to update_memory (close_video moves them)
+    _CARRIED = ("st_K", "st_V", "curr_Q", "curr_V")
+
+    def _check_family(self, cfg):
+        if cfg.MODEL_VOS == "deaot":
+            raise NotImplementedError("MultiVideoInferEngine runs the AOT models; DeAOT's gated propagation runs on "
+                                      "DeAOTMultiVideoInferEngine")
+
+    def _check_kernels(self):
+        """Refuse the knobs that select a kernel other than the batched entry points' (read at construction)."""
+        if E.LT_IMPL == "simt":
+            raise NotImplementedError("MultiVideoInferEngine runs the tensor-core long-term attention; AOTB_LT_IMPL=simt "
+                                      "selects the fp32 CUDA-core kernel")
+        if ops.CONV_IMPL == "simt":
+            raise NotImplementedError("MultiVideoInferEngine runs the tensor-core conv; AOTB_CONV_IMPL=simt selects the fp32 "
+                                      "CUDA-core conv")
+        if ops.LT_VARIANT != "tile":
+            raise NotImplementedError(f"MultiVideoInferEngine runs the default 'tile' layout of the long-term attention; "
+                                      f"AOTB_LT_VARIANT={ops.LT_VARIANT} selects another")
+        if E.LOCAL_IMPL != "tc":
+            raise NotImplementedError(f"MultiVideoInferEngine runs the tensor-core local attention; AOTB_LOCAL_IMPL="
+                                      f"{E.LOCAL_IMPL} selects a CUDA-core kernel")
+
     # ------------------------------------------------------------------ protocol
     def enable_kv_sharding(self, rank, world, group=None):
-        raise NotImplementedError("MultiVideoInferEngine pools bounded banks on one GPU; a bank sharded over GPUs is not "
-                                  "built for it")
+        raise NotImplementedError(f"{type(self).__name__} pools bounded banks on one GPU; a bank sharded over GPUs is not "
+                                  f"built for it")
 
     @property
     def videos(self):
@@ -104,7 +114,7 @@ class MultiVideoInferEngine:
             obj_nums = obj_nums[0]
         obj = int(obj_nums)
         if obj > self.max_obj_num:
-            raise NotImplementedError(f"MultiVideoInferEngine propagates at most {self.max_obj_num} objects per video (one "
+            raise NotImplementedError(f"{type(self).__name__} propagates at most {self.max_obj_num} objects per video (one "
                                       f"ID bank), got {obj}")
         return obj
 
@@ -161,10 +171,8 @@ class MultiVideoInferEngine:
         for src, dst in zip(embs[:3], pl.dec_in):
             ops.eltwise(ops.EW_COPY, src.reshape(-1, src.shape[3]), None, dst[b:b + 1].reshape(-1, dst.shape[3]), stream=st)
         self._copy_mask(b, mask, st)
-        P = self._P
-        ops.id_embed_runs_batched(pl.mask[b:b + 1], P.id_wp, P.id_b, pl.id_emb[b * N:(b + 1) * N], P.C, P.nid, P.id_k,
-                                  P.id_stride, P.id_pad, stream=st)
-        self._lstt(b, 1, embs[-1].reshape(N, P.C), st, ref=True)
+        self._id_embed(b, 1, st)
+        self._lstt(b, 1, embs[-1].reshape(N, self._P.C), st, ref=True)
         self._store(b, 1, st, flags=[1])
         s = self._slots[b]
         s["last_mem_step"] = s["frame_step"]
@@ -186,7 +194,7 @@ class MultiVideoInferEngine:
         for b, s in enumerate(self._slots):
             pl.frames[b:b + 1].copy_(frames[s["vid"]])
         embs = self._enc(pl.frames[:n], st).nhwc
-        splits = E.lt_splits(n * N, self._P.H, max(max(s["bank_len"] for s in self._slots), 1))
+        splits = self._splits(n * N, max(max(s["bank_len"] for s in self._slots), 1))
 
         def body():
             s2 = E._cur_stream()
@@ -254,11 +262,8 @@ class MultiVideoInferEngine:
 
         def body():
             s2 = E._cur_stream()
-            P, N = self._P, self._N
-            ops.id_embed_runs_batched(pl.mask[:n], P.id_wp, P.id_b, pl.id_emb[:n * N], P.C, P.nid, P.id_k, P.id_stride,
-                                      P.id_pad, stream=s2)
-            a = self._rows(0, n)
-            E.aot_fuse_memories(P, a, a.id_emb, a.st_K, a.st_V, s2)
+            self._id_embed(0, n, s2)
+            self._fuse_memories(self._rows(0, n), s2)
             self._store(0, n, s2)
         self.graphs.run(("upd", n), body)
         for s, f in zip(self._slots, flags):
@@ -278,8 +283,10 @@ class MultiVideoInferEngine:
                     rows(t, b, MN).copy_(rows(t, last, MN))
                 for t in (pl.bank_Kp[li], pl.bank_Vp[li]):
                     t[:, b * MN:(b + 1) * MN].copy_(t[:, last * MN:(last + 1) * MN])
-                for t in (pl.st_K[li], pl.st_V[li], pl.curr_Q[li], pl.curr_V[li]):
-                    rows(t, b, N).copy_(rows(t, last, N))
+                for name in self._CARRIED:
+                    t = pl.lstt[name][li]
+                    if t is not None:                              # DeAOT's curr_IDV[0]
+                        rows(t, b, N).copy_(rows(t, last, N))
             rows(pl.cat, b, N).copy_(rows(pl.cat, last, N))          # the decoder's inputs: LSTT output, encoder maps
             for t in pl.dec_in:
                 t[b].copy_(t[last])
@@ -299,13 +306,16 @@ class MultiVideoInferEngine:
     def _plan(self, refresh=False):
         if self._P is None or refresh:
             P = get_plan(self.AOT)
-            if P.C != 256 or P.C // P.H != 32:
-                raise NotImplementedError(f"MultiVideoInferEngine runs the 8 x 32 attention heads of the AOT models with "
-                                          f"256 channels, got {P.H} heads of {P.C // P.H}")
+            self._check_plan(P)
             if self._P is not None and P is not self._P:
                 self.graphs.clear()
             self._P = P
         return self._P
+
+    def _check_plan(self, P):
+        if P.C != 256 or P.C // P.H != 32:
+            raise NotImplementedError(f"MultiVideoInferEngine runs the 8 x 32 attention heads of the AOT models with "
+                                      f"256 channels, got {P.H} heads of {P.C // P.H}")
 
     def _ensure_pool(self, geom):
         P = self._P
@@ -332,16 +342,35 @@ class MultiVideoInferEngine:
         pl.tk = torch.zeros(S, dtype=torch.int32, device=dev)
         pl.wr = torch.zeros(S, dtype=torch.int32, device=dev)
         R = S * N
-        pl.lstt = E._aot_lstt_buffers(R, C, L, dev)
+        pl.lstt = self._lstt_buffers(R, C, L, dev)
         vars(pl).update(pl.lstt)
-        pl.bank_K, pl.bank_V = [f(S * M * N, C) for _ in range(L)], [f(S * M * N, C) for _ in range(L)]
-        pl.bank_Kp, pl.bank_Vp = [hz(P.H, S * M * N, 64) for _ in range(L)], [hz(P.H, S * M * N, 64) for _ in range(L)]
-        pl.Qp, pl.saKp, pl.saVp = hz(P.H, R, 64), hz(P.H, R, 64), hz(P.H, R, 64)
+        kc, vc = pl.st_K[0].shape[1], pl.st_V[0].shape[1]      # widths of a memory frame's K / V rows
+        pl.bank_K, pl.bank_V = [f(S * M * N, kc) for _ in range(L)], [f(S * M * N, vc) for _ in range(L)]
+        # packed operands, one 32-channel chunk per "head"
+        pl.bank_Kp, pl.bank_Vp = [hz(kc // 32, S * M * N, 64) for _ in range(L)], [hz(vc // 32, S * M * N, 64) for _ in range(L)]
+        pl.Qp, pl.saKp, pl.saVp = hz(kc // 32, R, 64), hz(kc // 32, R, 64), hz(vc // 32, R, 64)
         pl.part = {}
         pl.gn_ws = ops.groupnorm_workspace(S, 32, dev)
         pl.pos = E._pos_emb_sine(h, w, npf=C // 2).to(dev).repeat(S, 1).contiguous()
         pl.dec = {}
         self._pool, self._N, self._hw, self._geom = pl, N, (h, w), geom
+
+    def _lstt_buffers(self, rows, C, L, dev):
+        return E._aot_lstt_buffers(rows, C, L, dev)
+
+    def _splits(self, rows, tk):
+        """KV-split count of the batched long-term attention over `rows` query rows and at most tk live keys."""
+        return E.lt_splits(rows, self._P.H, tk)
+
+    def _id_embed(self, b, n, st):
+        """The ID embedding of slots [b, b + n)'s label maps into their id_emb rows."""
+        P, pl, N = self._P, self._pool, self._N
+        ops.id_embed_runs_batched(pl.mask[b:b + n], P.id_wp, P.id_b, pl.id_emb[b * N:(b + n) * N], P.C, P.nid, P.id_k,
+                                  P.id_stride, P.id_pad, ln_gamma=P.id_norm[0] if P.deaot else None,
+                                  ln_beta=P.id_norm[1] if P.deaot else None, stream=st)
+
+    def _fuse_memories(self, a, st):
+        E.aot_fuse_memories(self._P, a, a.id_emb, a.st_K, a.st_V, st)
 
     def _copy_mask(self, b, mask, st):
         m = mask.reshape(mask.shape[-2], mask.shape[-1]) if mask.dim() >= 2 else None
@@ -365,7 +394,7 @@ class MultiVideoInferEngine:
         r = slice(b * self._N, (b + n) * self._N)
         a = types.SimpleNamespace(gn_ws=self._pool.gn_ws)
         for k, t in self._pool.lstt.items():
-            setattr(a, k, t[r] if isinstance(t, torch.Tensor) else [u[r] for u in t])
+            setattr(a, k, t[r] if isinstance(t, torch.Tensor) else [None if u is None else u[r] for u in t])
         return a
 
     def _lstt(self, b, n, proj, st, ref, splits=None):
@@ -410,3 +439,73 @@ class MultiVideoInferEngine:
         x4, x8, x16 = (t[:n] for t in pl.dec_in)
         return E.fpn_decode(self._P, pl.cat[:n * self._N].view(n, *self._hw, -1), x4, x8, x16, pl.dec, pl.gn_ws,
                             E._cur_stream())
+
+
+class DeAOTMultiVideoInferEngine(MultiVideoInferEngine):
+    """DeAOTMultiVideoInferEngine(aot_model, max_videos=S, long_term_mem_max=M, gpu_id=0, long_term_mem_gap=None,
+    short_term_mem_skip=1, precision=None, long_term_mem_policy=None).
+
+    MultiVideoInferEngine for the DeAOT models: the same protocol, with per video the semantics of
+    DeAOTInferEngine(long_term_mem_max=M) with at most 10 objects.  Each frame's gated propagation (engine.deaot_lstt) runs
+    over the n open videos through the batched fused long-term / self-attention and the batched gated local attention."""
+
+    _CARRIED = MultiVideoInferEngine._CARRIED + ("curr_IDV",)
+
+    def _check_family(self, cfg):
+        if cfg.MODEL_VOS != "deaot":
+            raise NotImplementedError("DeAOTMultiVideoInferEngine runs the DeAOT models; AOT models run on "
+                                      "MultiVideoInferEngine")
+
+    def _check_kernels(self):
+        if ops.CONV_IMPL == "simt":
+            raise NotImplementedError("DeAOTMultiVideoInferEngine runs the tensor-core conv; AOTB_CONV_IMPL=simt selects "
+                                      "the fp32 CUDA-core conv")
+        if E.DEAOT_LT != "tc":
+            raise NotImplementedError(f"DeAOTMultiVideoInferEngine runs DeAOT's fused tensor-core attention; "
+                                      f"AOTB_DEAOT_LT={E.DEAOT_LT} selects another path")
+        if E.LOCAL_IMPL == "warp":
+            raise NotImplementedError("DeAOTMultiVideoInferEngine runs the tiled gated local attention; AOTB_LOCAL_IMPL=warp "
+                                      "selects the per-warp kernel")
+
+    def _check_plan(self, P):
+        if P.C != 256:
+            raise NotImplementedError(f"DeAOTMultiVideoInferEngine runs the gated attention of 128 key and 1024 value "
+                                      f"channels (256-channel models), got {P.C} channels")
+
+    def _lstt_buffers(self, rows, C, L, dev):
+        return E._deaot_gpm_buffers(rows, C, L, dev)
+
+    def _splits(self, rows, tk):
+        return E.gp_splits(rows, self._P.C, tk)
+
+    def _fuse_memories(self, a, st):
+        E.deaot_fuse_memories(self._P, a, a.id_emb, a.st_K, a.st_V, st)
+
+    def _lstt(self, b, n, proj, st, ref, splits=None):
+        """engine.deaot_lstt over slots [b, b + n): ref = the reference-frame form, else the propagation form over the
+        slots' banks.  Each attention step packs its operands and runs the batched fused kernel."""
+        P, pl, N = self._P, self._pool, self._N
+        a = self._rows(b, n)
+        MN = self.long_term_mem_max * N
+        exact = self.precision == "fp32"
+
+        def attend(Q, Kp, Vp, kv_stride, Tk, Tk_dev, out, splits, st):
+            ops.tc_pack_rows(Q, pl.Qp, 0, div=math.sqrt(Q.shape[1]), stream=st)      # Q / T (attention.py:672)
+            part = E._split_partials(pl.part, splits, n * N, 1, out.shape[1], out.device, cap_rows=self.max_videos * N) \
+                if splits > 1 else None
+            ops.gp_attention_tc_batched(pl.Qp, N, Kp, Vp, kv_stride, n, N, Tk=Tk, Tk_dev=Tk_dev, O=out, splits=splits,
+                                        exact=exact, part=part, stream=st)
+
+        def own(Q, K, V, out, st, long_term):
+            ops.tc_pack_rows(K, pl.saKp, 0, stream=st)
+            ops.tc_pack_rows(V, pl.saVp, 0, stream=st)
+            attend(Q, pl.saKp, pl.saVp, N, N, None, out, E.gp_splits(n * N, P.C, N), st)
+
+        def bank(li, Q, out, st):
+            attend(Q, pl.bank_Kp[li], pl.bank_Vp[li], MN, 0, pl.tk[b:b + n], out, splits, st)
+
+        def local(li, Q, K, V, out, st):
+            Lw = P.layers[li]
+            ops.local_gated_tile_batched(Q, K, V, Lw.relk_w, Lw.relk_b, out, *self._hw, n, stream=st)
+
+        E.deaot_lstt(P, a, proj, self._hw, n, a.st_K, a.st_V, a.id_emb if ref else None, own, bank, local, st)

@@ -974,6 +974,54 @@ def lt_attention_tc_batched(Qp, q_stride, Kp, Vp, kv_stride, n, N, Tk=0, Tk_dev=
     return O
 
 
+def gp_attention_tc_batched(Qp, q_stride, Kp, Vp, kv_stride, n, N, Tk=0, Tk_dev=None, O=None, splits=1, exact=True,
+                            part=None, stream=None):
+    """n DeAOT attentions in one launch (gp_attention_tc's kernel): problem b's queries are rows [b q_stride, b q_stride + N)
+    of Qp [4, q_rows, 64], its keys / values rows [b kv_stride, b kv_stride + Tk_dev[b]) of Kp [4, kv_rows, 64] / Vp [dv/32,
+    kv_rows, 64] (Tk_dev int32 [n], or Tk for all when None); O [n N, dv] receives rows [b N, (b + 1) N).  With splits > 1,
+    `part` = (Opart [splits, n N, dv], Mpart [splits, 1, n N], Lpart [splits, 1, n N]) and O receives their merge."""
+    q_rows, dv = Qp.shape[1], Vp.shape[0] * 32
+    if Qp.shape[0] != 4 or Kp.shape[0] != 4 or Vp.shape[1] != Kp.shape[1]:
+        raise AotbError(f"gp_attention_tc_batched: Qp / Kp must be [4, rows, 64] and Vp [dv/32, kv_rows, 64], got "
+                        f"{tuple(Qp.shape)}, {tuple(Kp.shape)}, {tuple(Vp.shape)}")
+    if splits > 1:
+        Op, Mp, Lp = part
+        _chk(Op, Mp, Lp)
+        if tuple(Op.shape) != (splits, n * N, dv) or tuple(Mp.shape) != (splits, 1, n * N) or Lp.shape != Mp.shape:
+            raise AotbError(f"gp_attention_tc_batched: partials must be [{splits}, {n * N}, {dv}] and [{splits}, 1, {n * N}], "
+                            f"got {tuple(Op.shape)}, {tuple(Mp.shape)}, {tuple(Lp.shape)}")
+    else:
+        Op = Mp = Lp = None
+    if Tk_dev is not None and (Tk_dev.dtype != torch.int32 or not Tk_dev.is_cuda or Tk_dev.numel() != n):
+        raise AotbError(f"gp_attention_tc_batched: Tk_dev must be an int32 CUDA tensor [{n}]")
+    if O is None or O.shape[0] != n * N or O.shape[1] != dv:
+        raise AotbError(f"gp_attention_tc_batched: O must be [{n * N}, {dv}]")
+    _chk(O)
+    check(lib().aotb_gp_attn_tc_batched_f16x2(Qp.data_ptr(), int(q_stride), q_rows, Kp.data_ptr(), Vp.data_ptr(),
+                                              int(kv_stride), Kp.shape[1], int(n), int(N), int(Tk),
+                                              Tk_dev.data_ptr() if Tk_dev is not None else None, dv,
+                                              _p(O) if splits == 1 else None, O.stride(0), _p(Op), _p(Mp), _p(Lp), int(splits),
+                                              (1 if exact else 0) | (4 if LT_SPIN else 0), _st(stream)),
+          "aotb_gp_attn_tc_batched_f16x2")
+    if splits > 1:
+        attn_merge(Op, Mp, Lp, O, 1, dv, stream=stream)
+    return O
+
+
+def local_gated_tile_batched(q, k, v, relk_w, relk_b, out, h, w, n, stream=None):
+    """local_gated_tile over n h x w maps stacked along the rows of q, k ([n h w, 128]), v and out ([n h w, 1024])."""
+    _chk(q, k, v, relk_w, relk_b, out)
+    if q.shape[1] != 128 or k.shape[1] != 128 or v.shape[1] != 1024 or out.shape[1] != 1024 or not relk_w.is_contiguous():
+        raise AotbError("local_gated_tile_batched: q / k [n hw, 128], v / out [n hw, 1024], contiguous relative_emb_k "
+                        "weights [225, 128]")
+    if any(t.shape[0] != n * h * w for t in (q, k, v, out)):
+        raise AotbError(f"local_gated_tile_batched: q, k, v and out need {n} x {h * w} rows")
+    check(lib().aotb_local_gated_tile_batched_f32(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(relk_w),
+                                                  _p(relk_b), _p(out), out.stride(0), h, w, int(n), _st(stream)),
+          "aotb_local_gated_tile_batched_f32")
+    return out
+
+
 def local_attention_tc_batched(q, k, v, relk_w, relk_b, relv_t, out, h, w, H, n, stream=None):
     """local_attention_tc over n h x w maps stacked along the rows of q, k, v and out ([n h w, ...] each)."""
     _chk(q, k, v, relk_w, relk_b, relv_t, out)

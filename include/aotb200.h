@@ -416,6 +416,21 @@ int aotb_bank_ring_store_batched(const float* k_src, int ldk, int k_cols, const 
 int aotb_ring_advance_batched(int* live, int* write, const int* store, int n, int rows, int cap_rows, int pinned_rows,
                               void* stream);
 
+/* ---- the same for DeAOT's gated propagation (DeAOTMultiVideoInferEngine), in the form above.
+ *   aotb_gp_attn_tc_batched_f16x2  (aotb_gp_attn_tc_f16x2; GatedPropagation.forward, networks/layers/attention.py:672-704, the
+ *       long-term and self-attention calls of networks/layers/transformer.py:614-653): queries at rows b q_stride of
+ *       Qp [4][q_rows][64], keys at rows b kv_stride of Kp [4][kv_rows][64], values of Vp [dv/32][kv_rows][64], live keys
+ *       Tk_dev[b] (int32 [n]; null: Tk for all); O [n N][ldo], or with splits > 1 partials Opart [splits][n N][dv],
+ *       Mpart / Lpart [splits][1][n N] for aotb_attn_merge_f32 (H = 1, d_v = dv) over n N rows.  exact bits 0 and 2.
+ *   aotb_local_gated_tile_batched_f32  (aotb_local_gated_tile_f32; LocalGatedPropagation.forward, attention.py:789-861):
+ *       map b = rows [b h w, (b + 1) h w) of q, k, v, out. */
+int aotb_gp_attn_tc_batched_f16x2(const void* Qp, int q_stride, int q_rows, const void* Kp, const void* Vp, int kv_stride,
+                                  int kv_rows, int n, int N, int Tk, const int* Tk_dev, int dv, float* O, int ldo, float* Opart,
+                                  float* Mpart, float* Lpart, int splits, int exact, void* stream);
+int aotb_local_gated_tile_batched_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                                      const float* relk_w, const float* relk_b, float* out, int ldo, int h, int w, int n,
+                                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,5 +1,5 @@
-"""Aggregate frames/s of n independent videos: (a) MultiVideoInferEngine, one batched pass per frame; (b) n AOTInferEngines
-on concurrent streams through engine.fork_join; (c) the same n engines one after another.  Per step: propagate + decode +
+"""Aggregate frames/s of n independent videos: (a) MultiVideoInferEngine (DeAOTMultiVideoInferEngine for a DeAOT model), one
+batched pass per frame; (b) n AOTInferEngines (DeAOTInferEngines) on concurrent streams through engine.fork_join; (c) the same n engines one after another.  Per step: propagate + decode +
 argmax + memory update, timed between CUDA events (every arm decodes stride-4 logits and runs the fused upsample + argmax
 kernel to the output size); the arms alternate in one session after an untimed pass each.
 Seeded random weights, 10 objects, long_term_mem_max 8, gap 5.  Prints one JSON line per (model, n, arm)."""
@@ -23,7 +23,7 @@ def main():
     a = ap.parse_args()
     from aot_benchmark_b200 import EngineConfig, build_vos_model
     from aot_benchmark_b200 import engine as E
-    from aot_benchmark_b200.multi_video import MultiVideoInferEngine
+    from aot_benchmark_b200.multi_video import DeAOTMultiVideoInferEngine, MultiVideoInferEngine
     from oracle import weights as OW
     H, W = (int(s) for s in a.size.split(","))
     out_size = (480, 854)
@@ -35,12 +35,14 @@ def main():
         model = build_vos_model(cfg.MODEL_VOS, cfg)
         model.load_state_dict(OW.build_state_dict(name, seed=0))
         model = model.cuda().eval()
+        deaot = cfg.MODEL_VOS == "deaot"
+        Multi, Single = (DeAOTMultiVideoInferEngine, E.DeAOTInferEngine) if deaot else (MultiVideoInferEngine, E.AOTInferEngine)
         g = torch.Generator(device="cuda").manual_seed(0)
         frame = torch.randn(1, 3, H, W, device="cuda", generator=g)
         mask = torch.randint(0, objs + 1, (1, 1, H, W), device="cuda", generator=g).float()
         for n in (int(s) for s in a.videos.split(",")):
-            multi = MultiVideoInferEngine(model, max_videos=n, long_term_mem_max=M, long_term_mem_gap=gap)
-            singles = [E.AOTInferEngine(model, long_term_mem_gap=gap, long_term_mem_max=M) for _ in range(n)]
+            multi = Multi(model, max_videos=n, long_term_mem_max=M, long_term_mem_gap=gap)
+            singles = [Single(model, long_term_mem_gap=gap, long_term_mem_max=M) for _ in range(n)]
             owner = type("Owner", (), {})()
 
             def run_multi(T):
