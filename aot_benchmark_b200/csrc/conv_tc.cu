@@ -77,11 +77,13 @@ struct ConvTcArgs {
     int spin;            // 1: mbarrier waits without the suspend hint
     int const_w;         // 1: no earlier kernel of the stream writes the weights (their first TMA loads precede pdl_wait)
     long long* prof;     // diagnostic: 12 clock64 stamps per CTA (see aotb_set_conv_tiling), or null
+    int htx, hti;        // halo path: 16-column tiles per map row, 8 x 16 tiles per image
 };
 
 constexpr int AOTB_CONV_CONST_WEIGHTS = 256;       // flag in the act argument (include/aotb200.h)
 static int g_conv_tiling = 0;      // aotb_set_conv_tiling
 static int g_conv_grid_cap = 0;    // aotb_set_conv_grid_cap (0: one CTA per SM)
+static int g_conv_halo = 1;        // aotb_set_conv_halo (0: never, 1: tile model, 2: every eligible launch)
 
 struct RowInfo { int pix_base, iy0, ix0, valid; };
 
@@ -146,14 +148,15 @@ __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefe
 // appears once.  G column groups per batch: every residual load of a batch is issued before its first use.  With one
 // group per batch (BN = 256, where 128 accumulators leave no room for more, and the rolled loop) each step would wait a
 // full L2 round trip for its residual; prefetch.global.L1 requests the groups PF steps ahead without registers.
+// r: output pixel of the thread's first row; its second row is pixel r + 8 (ok0 / ok1: the rows lie in the map).
 template <int BN, int ACT>
-__device__ __forceinline__ void conv_finish_frag(const ConvTcArgs& a, float* acc, const float* bs, int m0, int n0) {
+__device__ __forceinline__ void conv_finish_frag(const ConvTcArgs& a, float* acc, const float* bs, int r, bool ok0, bool ok1,
+                                                 int n0) {
     constexpr bool ROLL = ACT == ACT_GELU || ACT == ACT_SILU;
     constexpr int G = (ROLL || BN == 256) ? 1 : 8, NG = BN / 8, PF = 8;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int r = m0 + (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int lane = threadIdx.x & 31;
     const int c = (lane & 3) * 2;
-    const bool ok[2] = {r < a.M, r + 8 < a.M};
+    const bool ok[2] = {ok0, ok1};
     auto res_at = [&](int h, int k) { return a.res + (size_t)(r + 8 * h) * a.ldres + n0 + c + 8 * k; };
     auto prefetch = [&](int k) {
         if (G == 1 && a.res && k < NG) {
@@ -201,6 +204,18 @@ __device__ __forceinline__ void conv_finish_frag(const ConvTcArgs& a, float* acc
 #pragma unroll
                 for (int h = 0; h < 2; ++h) group(k0 + k, h, acc[4 * (k0 + k) + 2 * h], acc[4 * (k0 + k) + 2 * h + 1], rs[k][h]);
         }
+    }
+}
+
+template <int BN>
+__device__ __forceinline__ void conv_finish_act(const ConvTcArgs& a, float* acc, const float* bs, int r, bool ok0, bool ok1,
+                                                int n0) {
+    switch (a.act) {
+        case ACT_RELU: conv_finish_frag<BN, ACT_RELU>(a, acc, bs, r, ok0, ok1, n0); break;
+        case ACT_GELU: conv_finish_frag<BN, ACT_GELU>(a, acc, bs, r, ok0, ok1, n0); break;
+        case ACT_SILU: conv_finish_frag<BN, ACT_SILU>(a, acc, bs, r, ok0, ok1, n0); break;
+        case ACT_RELU6: conv_finish_frag<BN, ACT_RELU6>(a, acc, bs, r, ok0, ok1, n0); break;
+        default: conv_finish_frag<BN, ACT_NONE>(a, acc, bs, r, ok0, ok1, n0); break;
     }
 }
 
@@ -350,14 +365,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
                 // the bias / scale columns of tile j are visible; every consumer has finished tile j - 1, whose buffer
                 // tile j + 1 rewrites
                 asm volatile("bar.sync 1, 256;" ::: "memory");
-                const int m0 = tile_m0(j), n0 = tile_n0(j);
-                switch (a.act) {
-                    case ACT_RELU: conv_finish_frag<BN, ACT_RELU>(a, acc, bs, m0, n0); break;
-                    case ACT_GELU: conv_finish_frag<BN, ACT_GELU>(a, acc, bs, m0, n0); break;
-                    case ACT_SILU: conv_finish_frag<BN, ACT_SILU>(a, acc, bs, m0, n0); break;
-                    case ACT_RELU6: conv_finish_frag<BN, ACT_RELU6>(a, acc, bs, m0, n0); break;
-                    default: conv_finish_frag<BN, ACT_NONE>(a, acc, bs, m0, n0); break;
-                }
+                const int r = tile_m0(j) + warp * 16 + ((tid & 31) >> 2);
+                conv_finish_act<BN>(a, acc, bs, r, r < a.M, r + 8 < a.M, tile_n0(j));
                 if (tid == 0) { if (j == 0) stamp(8); stamp(9); }
             } else {
                 // every MMA of both warpgroups has completed before the staging tile overwrites the operand stages (a split-K
@@ -501,6 +510,235 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__
     if (tid == 0) stamp(7);
 }
 
+// ======================= stride-1 3x3 convolutions from one staged halo per 64-channel slice =======================
+// One tile = 8 x 16 output pixels of one image x BN channels; pixel row m of the tile (the accumulator row) is
+// (ty, tx) = (m / 16, m % 16), so consumer warp w (0-7) holds map row y0 + w.  For each 64-channel slice of Cin the
+// producer stages the tile's 10 x 18 input halo once, split into hi / lo fp16 (180 rows of 128 bytes per part, 16-byte
+// column c of halo pixel h at h * 128 + ((c ^ (h % 8)) << 4), so the eight rows an ldmatrix phase reads hit eight
+// different bank groups); pixels outside the image are stored as zeros, which is the padding.  The nine taps then read
+// their A fragments out of the halo with ldmatrix, each lane addressing the halo pixel of its output pixel shifted by
+// (ky, kx), and issue register-A wgmma: per chunk 4 k-steps x (Ah Wh + Al Wh + Ah Wl) as in conv_tc_kernel.
+// K runs slice-major, chunk (slice, tap) = K columns [tap * Cin + 64 slice, + 64) of the (ky, kx, ci) weight packing; with
+// Cin = 64 that is the order of conv_tc_kernel, whose outputs this kernel then reproduces bit for bit.
+//   warps 0-7   consumers.  Per chunk: ldmatrix of KG k-steps, wgmma_fence, their MMAs, wait (the A registers are reused),
+//               release the weight stage after the chunk and the halo after the slice's last ldmatrix; the finish as in
+//               the persistent conv_tc_kernel.
+//   warp 8      one lane streams the weight chunks by TMA into a STAGES ring (b_full / b_free).
+//   warps 9-11  halo producers (96 threads), two halo buffers (h_full / h_free): slice u + 1 -- of this or the next
+//               tile -- is staged while the taps of slice u run.
+constexpr int HALO_PIX = 10 * 18, HALO_PART_BYTES = HALO_PIX * 128;
+
+template <int BN, int STAGES, bool SPLIT>
+struct HaloSmem {
+    static constexpr int PARTS = SPLIT ? 2 : 1;
+    static constexpr int B_BYTES = BN * 128;
+    static constexpr int STAGE_BYTES = PARTS * B_BYTES;
+    static constexpr int HALO_BYTES = PARTS * HALO_PART_BYTES;
+    static constexpr int TOTAL = STAGES * STAGE_BYTES + 2 * HALO_BYTES + 2 * 2 * BN * 4 + (2 * STAGES + 4) * 8 + 1024;
+    static_assert(TOTAL <= 227 * 1024, "shared memory of one CTA");
+};
+
+template <int BN>
+__device__ __forceinline__ void wgmma_rs_conv(float* acc, const uint32_t* a, uint64_t b) {
+    if (BN == 256) wgmma_rs_n256(acc, a, b);
+    else if (BN == 128) wgmma_rs_n128(acc, a, b);
+    else wgmma_rs_n64(acc, a, b);
+}
+
+template <int BN, int STAGES, bool SPLIT>
+__global__ void __launch_bounds__(384, 1)
+conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const ConvTcArgs a) {
+    using SM = HaloSmem<BN, STAGES, SPLIT>;
+    // k-steps per wgmma group: their A fragments are live until the group's wait (8 registers per k-step when split),
+    // beside BN / 2 accumulators
+    constexpr int KG = BN < 256 ? 4 : SPLIT ? 1 : 2;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* halo = smem + STAGES * SM::STAGE_BYTES;                       // [2][PARTS][180][128 B]
+    float* bsm = reinterpret_cast<float*>(halo + 2 * SM::HALO_BYTES);     // [2][2][BN]: bias, scale of tiles j, j + 1
+    uint64_t* b_full = reinterpret_cast<uint64_t*>(bsm + 4 * BN);          // TMA transaction bytes
+    uint64_t* b_free = b_full + STAGES;                                   // 8 consumer-warp arrivals
+    uint64_t* h_full = b_free + STAGES;                                   // 96 producer-thread arrivals
+    uint64_t* h_free = h_full + 2;                                        // 8 consumer-warp arrivals
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int ntn = a.Cout / BN, ntiles = a.mtiles * ntn;
+    const int ntc = (int)blockIdx.x < ntiles ? (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+    const int ns = a.Cin >> 6, nloc = 9 * ns, nchk = ntc * nloc;
+    // tile j of this CTA: image b, top-left output pixel (y0, x0), first channel n0; the N tiles of one pixel tile are
+    // adjacent and every image has its own tile range
+    auto tile_of = [&](int j, int& b, int& y0, int& x0, int& n0) {
+        const int t = (int)blockIdx.x + j * (int)gridDim.x, mb = t / ntn;
+        n0 = (t - mb * ntn) * BN;
+        b = mb / a.hti;
+        const int r = mb - b * a.hti, ty = r / a.htx;
+        y0 = ty * 8;
+        x0 = (r - ty * a.htx) * 16;
+    };
+    pdl_trigger();
+    if (tid == 0) {
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_free[s], 8); }
+        for (int s = 0; s < 2; ++s) { mbar_init(&h_full[s], 96); mbar_init(&h_free[s], 8); }
+        fence_mbar_init();
+    }
+    __syncthreads();
+    const int npre = a.const_w ? min(STAGES, nchk) : 0;
+    auto issue_b = [&](int g) {
+        const int j = g / nloc, it = g - j * nloc, sl = it / 9, tap = it - sl * 9, s = g % STAGES;
+        int b, y0, x0, n0;
+        tile_of(j, b, y0, x0, n0);
+        uint8_t* Bh = smem + s * SM::STAGE_BYTES;
+        const int k0 = tap * a.Cin + sl * 64;
+        mbar_arrive_expect_tx(&b_full[s], SM::STAGE_BYTES);
+        tma_load_2d(Bh, &tmWh, &b_full[s], k0, n0);
+        if constexpr (SPLIT) tma_load_2d(Bh + SM::B_BYTES, &tmWl, &b_full[s], k0, n0);
+    };
+    if (tid == 256) {
+        tma_prefetch_desc(&tmWh);
+        if constexpr (SPLIT) tma_prefetch_desc(&tmWl);
+        for (int g = 0; g < npre; ++g) issue_b(g);
+    }
+    pdl_wait();         // activations / residual below were written by earlier kernels
+
+    const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
+    if (wg < 2) {
+        // ======================= consumers =======================
+        const uint64_t dB0 = smem_desc_sw128(smem_u32(smem));
+        // ldmatrix row of this lane: tile column (lane & 7) + 8 ((lane >> 3) & 1), 16-byte column half lane >> 4
+        const int lx = (lane & 7) + ((lane >> 3) & 1) * 8, lc = lane >> 4;
+        const uint32_t halo_s = smem_u32(halo);
+        int g = 0, u = 0;
+#pragma unroll 1
+        for (int j = 0; j < ntc; ++j) {
+            int b, y0, x0, n0;
+            tile_of(j, b, y0, x0, n0);
+            float acc[BN / 2];
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            float* bs = bsm + (j & 1) * 2 * BN;
+            if (tid < BN) {            // read by the finish after the K loop, behind the barrier below
+                bs[tid] = a.bias ? __ldg(a.bias + n0 + tid) : 0.f;
+                bs[BN + tid] = a.wscale ? __ldg(a.wscale + n0 + tid) : 1.f;
+            }
+#pragma unroll 1
+            for (int sl = 0; sl < ns; ++sl, ++u) {
+                const int hb = u & 1;
+                mbar_wait_cp(&h_full[hb], (u >> 1) & 1, a.spin);
+                const uint32_t hbase = halo_s + hb * SM::HALO_BYTES;
+#pragma unroll 1
+                for (int tap = 0; tap < 9; ++tap, ++g) {
+                    const int ky = tap / 3, kx = tap - ky * 3;
+                    const int hp = (warp + ky) * 18 + lx + kx;
+                    const uint32_t rowa = hbase + hp * 128, sw = hp & 7;
+                    const int s = g % STAGES;
+                    mbar_wait_cp(&b_full[s], (g / STAGES) & 1, a.spin);
+                    const uint64_t bh = dB0 + (uint64_t)((s * SM::STAGE_BYTES) >> 4), bl = bh + (uint64_t)(SM::B_BYTES >> 4);
+#pragma unroll
+                    for (int k0 = 0; k0 < 4; k0 += KG) {
+                        uint32_t ah[KG][4], al[KG][4];
+#pragma unroll
+                        for (int k = 0; k < KG; ++k) {
+                            const uint32_t ad = rowa + (((2 * (k0 + k) + lc) ^ sw) << 4);
+                            ldmatrix_x4(ah[k], ad);
+                            if constexpr (SPLIT) ldmatrix_x4(al[k], ad + HALO_PART_BYTES);
+                        }
+                        // the slice's last reads of the halo are in registers: the producer may restage it
+                        if (tap == 8 && k0 + KG == 4) mbar_arrive_warp(&h_free[hb]);
+                        reg_fence<BN / 2>(acc);
+                        wgmma_fence();
+#pragma unroll
+                        for (int k = 0; k < KG; ++k) {
+                            const int ks = k0 + k;
+                            wgmma_rs_conv<BN>(acc, ah[k], bh + 2 * ks);
+                            if constexpr (SPLIT) {
+                                wgmma_rs_conv<BN>(acc, al[k], bh + 2 * ks);
+                                wgmma_rs_conv<BN>(acc, ah[k], bl + 2 * ks);
+                            }
+                        }
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        reg_fence<BN / 2>(acc);
+#pragma unroll
+                        for (int k = 0; k < KG; ++k)       // the fragments stay allocated until the wait above
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) {
+                                asm volatile("" : "+r"(ah[k][i])::"memory");
+                                if constexpr (SPLIT) asm volatile("" : "+r"(al[k][i])::"memory");
+                            }
+                    }
+                    mbar_arrive_warp(&b_free[s]);
+                }
+            }
+            // the bias / scale columns of tile j are visible; every consumer has finished tile j - 1, whose buffer
+            // tile j + 1 rewrites
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            const int oy = y0 + warp, ox = x0 + (lane >> 2);
+            const int r = (b * a.H + oy) * a.W + ox;
+            conv_finish_act<BN>(a, acc, bs, r, oy < a.H && ox < a.W, oy < a.H && ox + 8 < a.W, n0);
+        }
+    } else if (warp == 8) {
+        // ======================= weight TMA =======================
+        if (lane == 0) {
+#pragma unroll 1
+            for (int g = npre; g < nchk; ++g) {
+                const int s = g % STAGES;
+                if (g >= STAGES) mbar_wait_cp(&b_free[s], ((g / STAGES) - 1) & 1, a.spin);
+                issue_b(g);
+            }
+        }
+    } else {
+        // ======================= halo producers =======================
+        // Thread p loads the 16-byte segment q = p % 16 (channels 4 q .. 4 q + 3 of the slice) of halo pixels p / 16 + 6 i,
+        // i = 0..29, in batches of NB loads in flight (two round trips to memory per slice; three at BN = 256, whose 128
+        // accumulators leave fewer registers).
+        const int p = tid - 288, q = p & 15, h0 = p >> 4;
+        const float4* in4 = reinterpret_cast<const float4*>(a.in);
+        int u = 0;
+#pragma unroll 1
+        for (int j = 0; j < ntc; ++j) {
+            int b, y0, x0, n0;
+            tile_of(j, b, y0, x0, n0);
+#pragma unroll 1
+            for (int sl = 0; sl < ns; ++sl, ++u) {
+                const int hb = u & 1;
+                if (u >= 2) mbar_wait_cp(&h_free[hb], ((u >> 1) - 1) & 1, a.spin);
+                uint8_t* hh = halo + hb * SM::HALO_BYTES;
+                const int c4 = sl * 16 + q;
+                constexpr int NB = BN == 256 ? 10 : 15;
+#pragma unroll 1
+                for (int i0 = 0; i0 < 30; i0 += NB) {
+                    float4 v[NB];
+#pragma unroll
+                    for (int i = 0; i < NB; ++i) {
+                        const int h = h0 + 6 * (i0 + i), hy = h / 18, hx = h - hy * 18;
+                        const int iy = y0 - 1 + hy, ix = x0 - 1 + hx;
+                        v[i] = (iy >= 0 && iy < a.H && ix >= 0 && ix < a.W)
+                                   ? __ldg(in4 + (((size_t)(b * a.H + iy) * a.W + ix) * a.ldin >> 2) + c4)
+                                   : make_float4(0.f, 0.f, 0.f, 0.f);
+                    }
+#pragma unroll
+                    for (int i = 0; i < NB; ++i) {
+                        const int h = h0 + 6 * (i0 + i);
+                        uint8_t* dst = hh + h * 128 + ((((q >> 1) ^ (h & 7))) << 4) + ((q & 1) << 3);
+                        const __half2 x0h = __floats2half2_rn(v[i].x, v[i].y), x1h = __floats2half2_rn(v[i].z, v[i].w);
+                        uint2 ph;
+                        ph.x = *reinterpret_cast<const uint32_t*>(&x0h); ph.y = *reinterpret_cast<const uint32_t*>(&x1h);
+                        *reinterpret_cast<uint2*>(dst) = ph;
+                        if constexpr (SPLIT) {
+                            const __half2 l0 = __floats2half2_rn(v[i].x - __low2float(x0h), v[i].y - __high2float(x0h));
+                            const __half2 l1 = __floats2half2_rn(v[i].z - __low2float(x1h), v[i].w - __high2float(x1h));
+                            uint2 pl;
+                            pl.x = *reinterpret_cast<const uint32_t*>(&l0); pl.y = *reinterpret_cast<const uint32_t*>(&l1);
+                            *reinterpret_cast<uint2*>(dst + HALO_PART_BYTES) = pl;
+                        }
+                    }
+                }
+                mbar_arrive(&h_full[hb]);
+            }
+        }
+    }
+}
+
 static int make_tmap_weights(CUtensorMap* out, const void* base, int Kpad, int Cout, int BN) {
     PFN_encodeTiled fn = tensor_map_encoder();
     if (!fn) return AOTB_ERR_CUDA;
@@ -558,6 +796,22 @@ static int launch_conv_tc(const CUtensorMap& th, const CUtensorMap& tl, const Co
                         : launch_conv_tc_as<BN, STAGES, SPLIT, true>(th, tl, a, st);
 }
 
+template <int BN, int STAGES, bool SPLIT>
+static int launch_halo(const CUtensorMap& th, const CUtensorMap& tl, const ConvTcArgs& a, cudaStream_t st) {
+    constexpr int smem = HaloSmem<BN, STAGES, SPLIT>::TOTAL;
+    static bool configured = false;
+    if (!configured) {
+        cudaError_t e = cudaFuncSetAttribute(conv3x3_halo_kernel<BN, STAGES, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (e != cudaSuccess) {
+            set_error("aotb_conv2d_nhwc_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+            return AOTB_ERR_CUDA;
+        }
+        configured = true;
+    }
+    launch_cluster(conv3x3_halo_kernel<BN, STAGES, SPLIT>, conv_grid(a, BN), dim3(384), smem, st, 1, th, tl, a);
+    return check_launch("aotb_conv2d_nhwc_tc");
+}
+
 }  // namespace tc
 }  // namespace aotb
 
@@ -572,6 +826,12 @@ extern "C" int aotb_set_conv_tiling(int mode) {
 extern "C" int aotb_set_conv_grid_cap(int ctas) {
     AOTB_REQUIRE(ctas >= 0, "aotb_set_conv_grid_cap: negative cap");
     tc::g_conv_grid_cap = ctas;
+    return AOTB_OK;
+}
+
+extern "C" int aotb_set_conv_halo(int mode) {
+    AOTB_REQUIRE(mode >= 0 && mode <= 2, "aotb_set_conv_halo: mode is 0, 1 or 2");
+    tc::g_conv_halo = mode;
     return AOTB_OK;
 }
 
@@ -629,8 +889,8 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     const int mt = cdiv(a.M, 128);
     int BN = 64, best_s = 1;
     const float kGather = 2.5f, kGather1 = 2.0f;
+    float best = 1e30f;
     if ((tc::g_conv_tiling & 1) == 0) {
-        float best = 1e30f;
         const int bns[3] = {256, 128, 64};
         const float t_mma[3] = {4.0f, 2.0f, 1.0f}, t_mma1[3] = {4.0f / 3, 2.0f / 3, 1.0f / 3};
         const float t_fin[3] = {8.0f, 4.0f, 2.0f};
@@ -675,6 +935,40 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     }
     a.spin = (tc::g_conv_tiling & 2) ? 1 : 0;
     a.prof = nullptr;
+    a.htx = a.hti = 0;
+    // Halo path (conv3x3_halo_kernel) for stride-1 3x3 pad-1 convolutions: 8 x 16 pixel tiles, each input element
+    // gathered and split once per 64-channel slice instead of once per tap, never split-K.  Its row of the model, in the
+    // same units: the consumers' MMAs bound a tile (the halo of a slice, 46 KB of fp32, is staged under the nine taps of
+    // the previous one), and the finish is not hidden, since both consumer warpgroups reach it together:
+    //     T = ramp + tpc * (nchunks * t_mma[BN] + t_finish[BN]),   tpc = ceil(pixel tiles * Cout / BN / 132)
+    // (single pass: t_mma at least 1).  Fitted with scripts/conv3x3_halo_sweep.py on an H100 80GB HBM3 (700 W), DESIGN 8.
+    // The policy takes it when it beats the best tiling of the chunked kernel above, split-K included.  A forced tiling
+    // keeps the chunked kernel unless aotb_set_conv_halo(2) forces the halo path (with the forced N tile).
+    const bool halo_ok = tc::g_conv_halo && KH == 3 && KW == 3 && stride == 1 && pad == 1 && Cin % 64 == 0 && force_s <= 1 &&
+                         (tc::g_conv_tiling & 4) == 0;
+    int hBN = BN;
+    bool use_halo = false;
+    if (halo_ok) {
+        a.htx = cdiv(W, 16);
+        a.hti = a.htx * cdiv(H, 8);
+        float best_h = 1e30f;
+        const int bns[3] = {256, 128, 64};
+        for (int bi = 0; bi < 3; ++bi) {
+            const int bn = bns[bi];
+            if (Cout % bn || (force_bn && bn != BN)) continue;
+            // single pass: a chunk costs at least one unit whatever its MMAs (the per-chunk waits and the A fragment loads)
+            const float tm = split ? bn / 64 : fmaxf(bn / 192.0f, 1.0f), tf = 2.0f * (bn / 64) * (bn == 256 && res ? 2.0f : 1.0f);
+            const float th = 3.0f + cdiv(B * a.hti * (Cout / bn), 132) * (a.nchunks * tm + tf);
+            if (th < best_h) { best_h = th; hBN = bn; }
+        }
+        use_halo = tc::g_conv_halo == 2 ||
+                   (!force_bn && !force_s && (tc::g_conv_tiling & 1) == 0 && best_h < best);
+    }
+    if (use_halo) {
+        BN = hBN;
+        a.splits = 1;
+        a.mtiles = B * a.hti;
+    }
     if (tc::g_conv_tiling & 4) {      // diagnostic stamps go to the caller's workspace
         const dim3 grid = tc::conv_grid(a, BN);
         const size_t need = (size_t)grid.x * grid.y * grid.z * 12 * sizeof(long long);
@@ -685,6 +979,17 @@ extern "C" int aotb_conv2d_nhwc_tc(const float* in, const void* wh, const void* 
     int rc;
     if ((rc = tc::make_tmap_weights(&th, wh, K, Cout, BN)) != AOTB_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
+    if (use_halo) {
+        if (!split) {
+            if (BN == 256) return tc::launch_halo<256, 4, false>(th, th, a, st);
+            if (BN == 128) return tc::launch_halo<128, 6, false>(th, th, a, st);
+            return tc::launch_halo<64, 8, false>(th, th, a, st);
+        }
+        if ((rc = tc::make_tmap_weights(&tl, wl, K, Cout, BN)) != AOTB_OK) return rc;
+        if (BN == 256) return tc::launch_halo<256, 2, true>(th, tl, a, st);
+        if (BN == 128) return tc::launch_halo<128, 3, true>(th, tl, a, st);
+        return tc::launch_halo<64, 4, true>(th, tl, a, st);
+    }
     if (!split) {             // the kernel never reads tmWl
         if (BN == 256) return tc::launch_conv_tc<256, 4, false>(th, th, a, st);
         if (BN == 128) return tc::launch_conv_tc<128, 6, false>(th, th, a, st);

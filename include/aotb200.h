@@ -41,6 +41,10 @@ int aotb_set_conv_tiling(int mode);
 /* Upper bound on the CTAs of a persistent (split-K free) aotb_conv2d_nhwc_tc launch; 0 (default) = one per SM.  The tile
  * order is static, so the output does not depend on the cap. */
 int aotb_set_conv_grid_cap(int ctas);
+/* Stride-1 3x3 pad-1 aotb_conv2d_nhwc_tc launches without split-K whose Cin is a multiple of 64 may run on the halo
+ * kernel: 8 x 16 pixel tiles whose input halo is staged once per 64-channel slice.  mode 1 (default): when the tile model
+ * favours it and aotb_set_conv_tiling forces no tiling; 0: never (every launch on the chunked kernel, to compare the two); 2: every such launch. */
+int aotb_set_conv_halo(int mode);
 
 /* nn.Conv2d (+ folded FrozenBatchNorm2d, + residual, + activation) as im2col-free implicit GEMM.
  * networks/encoders/resnet.py:34-54,140-157; networks/layers/normalization.py:30-43;

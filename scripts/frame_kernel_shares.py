@@ -9,7 +9,7 @@ kernels are not counted.  GPU only.
     python scripts/frame_kernel_shares.py OUT_DIR [--frames 20] [--model r50_aotl]
 
 Writes OUT_DIR/frame_kernel_shares.json (per kernel: launches and microseconds per frame, share of kernel time; the
-tensor-core conv family summed) and prints the table."""
+tensor-core conv family summed; the conv launches of one frame in order) and prints the table."""
 import argparse
 import collections
 import json
@@ -25,7 +25,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 import bench  # noqa: E402
 
-CONV_FAMILY = ("conv_tc_kernel",)
+CONV_FAMILY = ("conv_tc_kernel", "conv3x3_halo_kernel")
 
 
 def _short(name):
@@ -89,6 +89,13 @@ def main():
             a = agg[_short(ev["name"])]
             a[0] += 1
             a[1] += float(ev["dur"])
+    # the conv launches of one frame in launch order (every frame launches the same sequence), time averaged over frames
+    convs = sorted((ev for ev in trace.get("traceEvents", [])
+                    if ev.get("cat") == "kernel" and "dur" in ev and any(f in ev["name"] for f in CONV_FAMILY)),
+                   key=lambda ev: ev["ts"])
+    per = len(convs) // n if n else 0
+    conv_launches = [{"kernel": _short(convs[i]["name"]), "grid": convs[i].get("args", {}).get("grid"),
+                      "us": round(sum(float(convs[i + f * per]["dur"]) for f in range(n)) / n, 2)} for i in range(per)]
     total = sum(v[1] for v in agg.values())
     rows = [{"kernel": k, "launches_per_frame": round(c / n, 2), "us_per_frame": round(t / n, 2),
              "share": round(t / total, 4) if total else 0.0}
@@ -100,7 +107,7 @@ def main():
            "conv_tc_family": {"us_per_frame": round(sum(r["us_per_frame"] for r in conv), 2),
                               "share": round(sum(r["share"] for r in conv), 4),
                               "launches_per_frame": round(sum(r["launches_per_frame"] for r in conv), 2)},
-           "kernels": rows}
+           "kernels": rows, "conv_launches_per_frame": conv_launches}
     os.makedirs(args.out_dir, exist_ok=True)
     json.dump(out, open(os.path.join(args.out_dir, "frame_kernel_shares.json"), "w"), indent=1)
     print(f"gpu: {out['gpu']}; kernel time {out['kernel_us_per_frame']:.1f} us/frame over {n} frames; "
