@@ -7,6 +7,7 @@ Public surface (mirrors the reference's seam, SURVEY 8b):
     TTAInferEngine(aot_model, ...)        networks/managers/evaluator.py:265-446 with TEST_FLIP / TEST_MULTISCALE
     MultiVideoInferEngine(aot_model, ...) several independent videos propagated in one batched pass per frame
     DeAOTMultiVideoInferEngine(...)       the same for the DeAOT models
+    MultiVideoTTAInferEngine(...)         TTAInferEngine over several videos, one batched pass per scale per frame
 """
 from .configs import EngineConfig  # noqa: F401
 from .model import build_vos_model  # noqa: F401
@@ -24,4 +25,7 @@ def __getattr__(name):
     if name in ("MultiVideoInferEngine", "DeAOTMultiVideoInferEngine"):
         from . import multi_video
         return getattr(multi_video, name)
+    if name == "MultiVideoTTAInferEngine":
+        from .multi_video_tta import MultiVideoTTAInferEngine
+        return MultiVideoTTAInferEngine
     raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

@@ -268,11 +268,123 @@ __device__ __forceinline__ float tta_sample(const float* __restrict__ b, int w, 
     return hy * (hx * b[y0 * w + x0] + lx * b[y0 * w + x1]) + ly * (hx * b[y1 * w + x0] + lx * b[y1 * w + x1]);
 }
 
+// Up to TTA_BATCH videos (merge) or lanes (feedback) per launch, one per blockIdx.y; the entry points launch once per chunk.
+constexpr int TTA_BATCH = 32;
+
+struct TTAMergeBatchArgs {
+    const float* logits[8];     // per augmentation: its scale's decoder output [lanes][h][w][NC]
+    int h[8], w[8];
+    int flip[8];
+    int lane[TTA_BATCH][8];     // video b's lane in augmentation e's map
+    int obj[TTA_BATCH];
+    const float* new_label[TTA_BATCH];
+};
+
+// Tap loaders of the two TTA bodies below.  A loader gives a map's channel c blended at the four bilinear taps with
+// tta_sample's arithmetic, so a body never sees the logit layout.
+//   NCHW forms (the one-video kernels): masked low-resolution maps [NC][h][w].
+//   NHWC forms (the batched kernels): one lane of a multi-video decoder's output [lanes][h][w][NC], with the post-processing
+//   mask applied at every tap: a channel above the video's object count reads -1e10, the value aotb_logits_postproc_f32
+//   writes, and blended with tta_sample's roundings, so every sampled logit is bit for bit the one-video form's.
+__device__ __forceinline__ float tta_sample_nhwc(const float* __restrict__ b, int w, int NC, int c, int obj, int y0, int y1,
+                                                 int x0, int x1, float ly, float lx) {
+    auto tap = [&](int y, int x) { return c > obj ? -1e10f : __ldg(b + ((y * w + x) * NC + c)); };   // a lane < 2^31
+    const float hy = 1.f - ly, hx = 1.f - lx;
+    // tta_sample's blend with its contraction spelled out: nvcc compiles tta_sample in the one-video kernels to
+    // fma(hx, v0, lx * v1) per row and fma(hy, row0, ly * row1) across rows, and left to itself it contracts this copy the
+    // other way round at some sites, one ulp apart.
+    const float r0 = __fmaf_rn(hx, tap(y0, x0), __fmul_rn(lx, tap(y0, x1)));
+    const float r1 = __fmaf_rn(hx, tap(y1, x0), __fmul_rn(lx, tap(y1, x1)));
+    return __fmaf_rn(hy, r0, __fmul_rn(ly, r1));
+}
+
+// One map's channels: c -> channel c blended at the taps.
+struct TTANchwMap {
+    const float* lo;
+    size_t plane;
+    int w;
+    __device__ __forceinline__ float operator()(int c, int y0, int y1, int x0, int x1, float ly, float lx) const {
+        return tta_sample(lo + c * plane, w, y0, y1, x0, x1, ly, lx);
+    }
+};
+
+struct TTANhwcMap {
+    const float* b;             // the lane's [h][w][NC]
+    int w, NC, obj;
+    __device__ __forceinline__ float operator()(int c, int y0, int y1, int x0, int x1, float ly, float lx) const {
+        return tta_sample_nhwc(b, w, NC, c, obj, y0, y1, x0, x1, ly, lx);
+    }
+};
+
+struct TTAMergeNhwc {           // video b's lanes of E augmentations' maps
+    const TTAMergeBatchArgs& a;
+    int b, NC;
+    __device__ __forceinline__ int h(int e) const { return a.h[e]; }
+    __device__ __forceinline__ int w(int e) const { return a.w[e]; }
+    __device__ __forceinline__ int flip(int e) const { return a.flip[e]; }
+    __device__ __forceinline__ TTANhwcMap channels(int e) const {
+        return TTANhwcMap{a.logits[e] + (size_t)a.lane[b][e] * a.h[e] * a.w[e] * NC, a.w[e], NC, a.obj[b]};
+    }
+    __device__ __forceinline__ float operator()(int e, int c, int y0, int y1, int x0, int x1, float ly, float lx) const {
+        return channels(e)(c, y0, y1, x0, x1, ly, lx);
+    }
+};
+
+struct TTAFeedbackNchw {        // one map, or none (lo null)
+    const float* lo;
+    int h, w;
+    __device__ __forceinline__ bool live() const { return lo; }
+    __device__ __forceinline__ TTANchwMap channels() const { return TTANchwMap{lo, (size_t)h * w, w}; }
+};
+
+struct TTAFeedbackNhwc {        // one lane, or none (lane null)
+    TTANhwcMap lane;
+    __device__ __forceinline__ bool live() const { return lane.b; }
+    __device__ __forceinline__ const TTANhwcMap& channels() const { return lane; }
+};
+
 // evaluator.py:332-361: per output pixel, every augmentation's upsampled logits (read at the mirrored column for a flipped
 // one, :336-337) -> softmax over NC (:339) -> mean over the augmentations in order (:355-358) -> first argmax (:359-361),
 // then the new-object overlay n != 0 ? n : label (:363-369).  The mean probabilities go to prob [NC][H][W] when it is given.
 // Three passes over the channels per augmentation (max, sum, probability): the E x NC logits stay in L1 / L2, nothing but the
-// label (and the optional probabilities) is written.
+// label (and the optional probabilities) is written.  This is pixel i of one video.
+template <class Maps>
+__device__ __forceinline__ void tta_merge_pixel(const Maps& a, int E, int NC, int Ho, int Wo, int align, int i, int total,
+                                                float inv_e, const float* __restrict__ new_label, float* __restrict__ label,
+                                                float* __restrict__ prob) {
+    const int oy = i / Wo, ox = i - oy * Wo;
+    int y0[8], y1[8], x0[8], x1[8];
+    float ly[8], lx[8], m[8], s[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+        if (e < E) {
+            bl_src(oy, a.h(e), Ho, align, y0[e], y1[e], ly[e]);
+            bl_src(a.flip(e) ? Wo - 1 - ox : ox, a.w(e), Wo, align, x0[e], x1[e], lx[e]);
+            const auto ch = a.channels(e);
+            float mx = -INFINITY;
+            for (int c = 0; c < NC; ++c) mx = fmaxf(mx, ch(c, y0[e], y1[e], x0[e], x1[e], ly[e], lx[e]));
+            float sum = 0.f;
+            for (int c = 0; c < NC; ++c) sum += expf(ch(c, y0[e], y1[e], x0[e], x1[e], ly[e], lx[e]) - mx);
+            m[e] = mx;
+            s[e] = sum;
+        }
+    }
+    float best = -INFINITY;
+    int bi = 0;
+    for (int c = 0; c < NC; ++c) {
+        float acc = 0.f;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            if (e < E) acc += expf(a(e, c, y0[e], y1[e], x0[e], x1[e], ly[e], lx[e]) - m[e]) / s[e];
+        }
+        const float p = acc * inv_e;
+        if (prob) prob[(size_t)c * total + i] = p;
+        if (p > best) { best = p; bi = c; }
+    }
+    const float n = new_label ? new_label[i] : 0.f;
+    label[i] = n != 0.f ? n : (float)bi;
+}
+
 __global__ void tta_merge_kernel(const TTAArgs a, int E, int NC, int Ho, int Wo, int align,
                                  const float* __restrict__ new_label, float* __restrict__ label, float* __restrict__ prob) {
     pdl_sync();
@@ -318,41 +430,82 @@ __global__ void tta_merge_kernel(const TTAArgs a, int E, int NC, int Ho, int Wo,
     }
 }
 
+// tta_merge_kernel over n videos: video b = blockIdx.y reads its own lane of every augmentation's map, masked at its own
+// object count, and writes label [b][H][W] (and prob [b][NC][H][W]).
+__global__ void tta_merge_batched_kernel(const TTAMergeBatchArgs a, int E, int NC, int Ho, int Wo, int align,
+                                         float* __restrict__ label, float* __restrict__ prob) {
+    pdl_sync();
+    const int b = blockIdx.y;
+    const int total = Ho * Wo;
+    const float inv_e = 1.f / (float)E;
+    float* lb = label + (size_t)b * total;
+    float* pb = prob ? prob + (size_t)b * NC * total : nullptr;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x)
+        tta_merge_pixel(TTAMergeNhwc{a, b, NC}, E, NC, Ho, Wo, align, i, total, inv_e, a.new_label[b], lb, pb);
+}
+
 // evaluator.py:346-353, :363-422 for one augmentation: the label its engine stores in memory.  For input pixel (y, x) the
 // nearest source (sy, sx) at the output size follows nearest_kernel; base = argmax softmax of the upsampled logits at (sy, sx)
 // in the augmentation's own orientation (the flip of :336-337 and the flip back of :373-376 / :402-406 cancel), n = the
 // new-object label at the mirrored column for a flipped augmentation (mirror at output size first, then nearest: the two do not
-// commute), out = n != 0 ? n : base.  No logits: base = 0 (the first frame's label, :315-319); no new label: n = 0.
+// commute), out = n != 0 ? n : base.  No logits: base = 0 (the first frame's label, :315-319); no new label: n = 0.  This is
+// input pixel i of one augmentation.
+template <class Map>
+__device__ __forceinline__ void tta_feedback_pixel(const Map& lo, int h, int w, int NC, int H, int W, int align, int flip,
+                                                   const float* __restrict__ new_label, float* __restrict__ out, int i,
+                                                   int Wi, float sy, float sx) {
+    const int oy = i / Wi, ox = i - oy * Wi;
+    int iy = (int)floorf(oy * sy), ix = (int)floorf(ox * sx);
+    iy = iy < H - 1 ? iy : H - 1;
+    ix = ix < W - 1 ? ix : W - 1;
+    int base = 0;
+    if (lo.live()) {
+        int y0, y1, x0, x1;
+        float ly, lx;
+        bl_src(iy, h, H, align, y0, y1, ly);
+        bl_src(ix, w, W, align, x0, x1, lx);
+        const auto ch = lo.channels();
+        float mx = -INFINITY;
+        for (int c = 0; c < NC; ++c) mx = fmaxf(mx, ch(c, y0, y1, x0, x1, ly, lx));
+        float sum = 0.f;
+        for (int c = 0; c < NC; ++c) sum += expf(ch(c, y0, y1, x0, x1, ly, lx) - mx);
+        float best = -INFINITY;
+        for (int c = 0; c < NC; ++c) {
+            const float p = expf(ch(c, y0, y1, x0, x1, ly, lx) - mx) / sum;
+            if (p > best) { best = p; base = c; }
+        }
+    }
+    const float n = new_label ? new_label[(size_t)iy * W + (flip ? W - 1 - ix : ix)] : 0.f;
+    out[i] = n != 0.f ? n : (float)base;
+}
+
 __global__ void tta_feedback_kernel(const float* __restrict__ lo, int h, int w, int NC, int H, int W, int align, int flip,
                                     const float* __restrict__ new_label, float* __restrict__ out, int Hi, int Wi) {
     pdl_sync();
     const int total = Hi * Wi;
     const float sy = (float)H / (float)Hi, sx = (float)W / (float)Wi;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-        const int oy = i / Wi, ox = i - oy * Wi;
-        int iy = (int)floorf(oy * sy), ix = (int)floorf(ox * sx);
-        iy = iy < H - 1 ? iy : H - 1;
-        ix = ix < W - 1 ? ix : W - 1;
-        int base = 0;
-        if (lo) {
-            int y0, y1, x0, x1;
-            float ly, lx;
-            bl_src(iy, h, H, align, y0, y1, ly);
-            bl_src(ix, w, W, align, x0, x1, lx);
-            const size_t plane = (size_t)h * w;
-            float mx = -INFINITY;
-            for (int c = 0; c < NC; ++c) mx = fmaxf(mx, tta_sample(lo + c * plane, w, y0, y1, x0, x1, ly, lx));
-            float sum = 0.f;
-            for (int c = 0; c < NC; ++c) sum += expf(tta_sample(lo + c * plane, w, y0, y1, x0, x1, ly, lx) - mx);
-            float best = -INFINITY;
-            for (int c = 0; c < NC; ++c) {
-                const float p = expf(tta_sample(lo + c * plane, w, y0, y1, x0, x1, ly, lx) - mx) / sum;
-                if (p > best) { best = p; base = c; }
-            }
-        }
-        const float n = new_label ? new_label[(size_t)iy * W + (flip ? W - 1 - ix : ix)] : 0.f;
-        out[i] = n != 0.f ? n : (float)base;
-    }
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x)
+        tta_feedback_pixel(TTAFeedbackNchw{lo, h, w}, h, w, NC, H, W, align, flip, new_label, out, i, Wi, sy, sx);
+}
+
+struct TTAFeedbackBatchArgs {
+    int obj[TTA_BATCH];
+    int flip[TTA_BATCH];
+    const float* new_label[TTA_BATCH];
+};
+
+// tta_feedback_kernel over n lanes of one multi-video pool: lane k = blockIdx.y reads its rows of the decoder output
+// [lanes][h][w][NC] (masked at its object count; lg null: the no-logits form) and writes its memory label into out [k][Hi][Wi].
+__global__ void tta_feedback_batched_kernel(const float* __restrict__ lg, int h, int w, int NC, int H, int W, int align,
+                                            const TTAFeedbackBatchArgs a, float* __restrict__ out, int Hi, int Wi) {
+    pdl_sync();
+    const int k = blockIdx.y;
+    const int total = Hi * Wi;
+    const float sy = (float)H / (float)Hi, sx = (float)W / (float)Wi;
+    const TTAFeedbackNhwc lane{{lg ? lg + (size_t)k * h * w * NC : nullptr, w, NC, a.obj[k]}};
+    float* ok = out + (size_t)k * total;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x)
+        tta_feedback_pixel(lane, h, w, NC, H, W, align, a.flip[k], a.new_label[k], ok, i, Wi, sy, sx);
 }
 
 
@@ -630,6 +783,65 @@ extern "C" int aotb_tta_feedback_f32(const float* logits, int h, int w, int NC, 
     launch(tta_feedback_kernel, dim3(cdiv(Hi * Wi, 256)), dim3(256), 0, (cudaStream_t)stream, logits, h, w, NC, H, W,
            align_corners, flip ? 1 : 0, new_label, out, Hi, Wi);
     return check_launch("aotb_tta_feedback_f32");
+}
+
+extern "C" int aotb_tta_merge_batched_f32(const float* const* logits, const int* sizes, const int* flips, int n_augs,
+                                          const int* lanes, const int* obj_nums, int n, int NC, int H, int W,
+                                          int align_corners, const float* const* new_labels, float* label, float* pred_prob,
+                                          void* stream) {
+    AOTB_REQUIRE(logits && sizes && flips && lanes && obj_nums && label && n > 0 && NC > 0 && H > 0 && W > 0,
+                 "aotb_tta_merge_batched_f32: bad args");
+    AOTB_REQUIRE(n_augs >= 1 && n_augs <= 8, "aotb_tta_merge_batched_f32: 1 to 8 augmentations (got %d)", n_augs);
+    TTAMergeBatchArgs a;
+    for (int e = 0; e < 8; ++e) {
+        const bool live = e < n_augs;
+        a.logits[e] = live ? logits[e] : nullptr;
+        a.h[e] = live ? sizes[2 * e] : 1;
+        a.w[e] = live ? sizes[2 * e + 1] : 1;
+        a.flip[e] = live ? (flips[e] != 0) : 0;
+        AOTB_REQUIRE(!live || (a.logits[e] && a.h[e] > 0 && a.w[e] > 0), "aotb_tta_merge_batched_f32: augmentation %d: bad map",
+                     e);
+        AOTB_REQUIRE(!live || (size_t)a.h[e] * a.w[e] * NC < (1u << 31), "aotb_tta_merge_batched_f32: augmentation %d: lane "
+                     "too large", e);
+    }
+    const size_t plane = (size_t)H * W;
+    int launches = 0;
+    for (int v0 = 0; v0 < n; v0 += TTA_BATCH, ++launches) {
+        const int nb = n - v0 < TTA_BATCH ? n - v0 : TTA_BATCH;
+        for (int b = 0; b < nb; ++b) {
+            for (int e = 0; e < 8; ++e) {
+                a.lane[b][e] = e < n_augs ? lanes[(size_t)(v0 + b) * n_augs + e] : 0;
+                AOTB_REQUIRE(a.lane[b][e] >= 0, "aotb_tta_merge_batched_f32: video %d: negative lane", v0 + b);
+            }
+            a.obj[b] = obj_nums[v0 + b];
+            a.new_label[b] = new_labels ? new_labels[v0 + b] : nullptr;
+        }
+        launch(tta_merge_batched_kernel, dim3(cdiv(H * W, 256), nb), dim3(256), 0, (cudaStream_t)stream, a, n_augs, NC, H, W,
+               align_corners, label + v0 * plane, pred_prob ? pred_prob + v0 * NC * plane : nullptr);
+    }
+    return check_launch("aotb_tta_merge_batched_f32", launches);
+}
+
+extern "C" int aotb_tta_feedback_batched_f32(const float* logits, int h, int w, int NC, int n_lanes, const int* obj_nums,
+                                             const int* flips, const float* const* new_labels, int H, int W,
+                                             int align_corners, float* out, int Hi, int Wi, void* stream) {
+    AOTB_REQUIRE(out && flips && n_lanes > 0 && H > 0 && W > 0 && Hi > 0 && Wi > 0, "aotb_tta_feedback_batched_f32: bad args");
+    AOTB_REQUIRE(!logits || (obj_nums && h > 0 && w > 0 && NC > 0 && (size_t)h * w * NC < (1u << 31)),
+                 "aotb_tta_feedback_batched_f32: bad logit map");
+    const size_t lane = (size_t)h * w * NC, plane = (size_t)Hi * Wi;
+    TTAFeedbackBatchArgs a;
+    int launches = 0;
+    for (int k0 = 0; k0 < n_lanes; k0 += TTA_BATCH, ++launches) {
+        const int nb = n_lanes - k0 < TTA_BATCH ? n_lanes - k0 : TTA_BATCH;
+        for (int k = 0; k < nb; ++k) {
+            a.obj[k] = obj_nums ? obj_nums[k0 + k] : 0;
+            a.flip[k] = flips[k0 + k] != 0;
+            a.new_label[k] = new_labels ? new_labels[k0 + k] : nullptr;
+        }
+        launch(tta_feedback_batched_kernel, dim3(cdiv(Hi * Wi, 256), nb), dim3(256), 0, (cudaStream_t)stream,
+               logits ? logits + k0 * lane : nullptr, h, w, NC, H, W, align_corners, a, out + k0 * plane, Hi, Wi);
+    }
+    return check_launch("aotb_tta_feedback_batched_f32", launches);
 }
 
 

@@ -211,9 +211,8 @@ class MultiVideoInferEngine:
         over the n videos is one graph keyed on n; each video's logit post-processing (masking the ids above its object
         count, upsampling) follows it as an eager launch, so object counts that change as videos open, close or gain objects
         need no new graph."""
-        n = len(self._slots)
         size = None if output_size is None else (int(output_size[0]), int(output_size[1]))
-        lg = self.graphs.run(("dec", n), lambda: self._decode(n))
+        lg = self.decode_nhwc()
         st = E._cur_stream()
         h4, w4, NC = lg.shape[1], lg.shape[2], lg.shape[3]
         self._last_lowres, out = [], {}
@@ -224,6 +223,13 @@ class MultiVideoInferEngine:
             self._last_lowres.append(lo)
             out[s["vid"]] = lo if up is None else up
         return out
+
+    @E._in_precision
+    def decode_nhwc(self):
+        """The decoder over the n open videos -> their raw logits [n, h/4, w/4, 11] (NHWC, slot order, no object-count
+        mask): a static buffer the next decode overwrites.  decode_current_logits post-processes it per video."""
+        n = len(self._slots)
+        return self.graphs.run(("dec", n), lambda: self._decode(n))
 
     def decode_labels(self, output_size=None):
         """decode_current_logits fused with the argmax of each video's upsampled logits -> {vid: label [1, H, W] int64}."""
@@ -244,16 +250,28 @@ class MultiVideoInferEngine:
         if set(labels) != set(self.videos):
             raise ValueError(f"update_memory needs a label map for exactly the open videos {sorted(self.videos)}, got "
                              f"{sorted(labels)}")
-        n, pl = len(self._slots), self._pool
         st = E._cur_stream()
-        flags = []
         for b, s in enumerate(self._slots):
+            self._copy_mask(b, labels[s["vid"]], st)
+        self.update_memory_from_masks(skip_long_term_update)
+
+    def mask_rows(self):
+        """The open videos' label-map rows [n, H, W] at the network input size (slot order), which update_memory fills and
+        update_memory_from_masks reads."""
+        return self._pool.mask[:len(self._slots)]
+
+    @E._in_precision
+    def update_memory_from_masks(self, skip_long_term_update=False):
+        """update_memory on the label maps already in mask_rows() (written on the current stream): every video's
+        short-term memory, and the long-term bank of each video whose own gap has passed since its last memory frame."""
+        n, pl = len(self._slots), self._pool
+        flags = []
+        for s in self._slots:
             store = 0
             if s["frame_step"] - s["last_mem_step"] >= s["gap"]:
                 store = 0 if skip_long_term_update else 1
                 s["last_mem_step"] = s["frame_step"]
             flags.append(store)
-            self._copy_mask(b, labels[s["vid"]], st)
         host = torch.tensor(flags, dtype=torch.int32)
         if pl.flags.is_cuda:
             # pinned by the caching host allocator, which keeps the block until the asynchronous copy has run: no host sync

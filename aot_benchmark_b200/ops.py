@@ -708,6 +708,84 @@ def tta_feedback(logits, out, output_size, align_corners, flip, new_label=None, 
     return out
 
 
+def _label_maps(name, ts, n, H, W):
+    """n optional contiguous [H, W] maps -> a ctypes pointer array (None when every entry is None)."""
+    import ctypes
+    if ts is None or all(t is None for t in ts):
+        return None
+    if len(ts) != n:
+        raise AotbError(f"{name}: one entry per map, got {len(ts)} for {n}")
+    for t in ts:
+        _chk(t)
+        if t is not None and (t.numel() != H * W or not t.is_contiguous() or tuple(t.shape[-2:]) != (H, W)):
+            raise AotbError(f"{name}: each map must be one contiguous [{H}, {W}] map, got {tuple(t.shape)}")
+    return (ctypes.c_void_p * n)(*[_p(t) for t in ts])
+
+
+def tta_merge_batched(logits, flips, lanes, obj_nums, label, align_corners, new_labels=None, prob=None, stream=None):
+    """tta_merge over n videos in one launch, reading the multi-video decoders' outputs directly.  logits = E (1..8) NHWC maps
+    [lanes_e, h_e, w_e, NC] (one NC); lanes [n][E]: video b's lane in each map; obj_nums [n]: ids above obj_nums[b] are masked
+    as logits_postproc masks them; label [n, H, W] (leading dims of size 1 allowed between); prob [n, NC, H, W] or None;
+    new_labels: n [H, W] overlays or None entries.  Video b's label and probabilities are bit for bit logits_postproc +
+    tta_merge on its lanes."""
+    import ctypes
+    _chk(label, prob, *logits)
+    E, n = len(logits), len(lanes)
+    if not 1 <= E <= 8 or len(flips) != E:
+        raise AotbError(f"tta_merge_batched: 1 to 8 logit maps with one flip bit each, got {E} maps and {len(flips)} flips")
+    if n < 1 or len(obj_nums) != n or any(len(r) != E for r in lanes):
+        raise AotbError(f"tta_merge_batched: lanes [n][{E}] and obj_nums [n] for n >= 1 videos")
+    NC = int(logits[0].shape[-1])
+    for e, t in enumerate(logits):
+        if t.dim() != 4 or not t.is_contiguous() or t.shape[-1] != NC:
+            raise AotbError(f"tta_merge_batched: logits must be contiguous NHWC [lanes, h, w, {NC}], got {tuple(t.shape)}")
+        if any(not 0 <= r[e] < t.shape[0] for r in lanes):
+            raise AotbError(f"tta_merge_batched: augmentation {e}: lane out of [0, {t.shape[0]})")
+    H, W = label.shape[-2:]
+    if label.numel() != n * H * W or not label.is_contiguous():
+        raise AotbError(f"tta_merge_batched: label must be contiguous [{n}, {H}, {W}], got {tuple(label.shape)}")
+    if prob is not None and (prob.numel() != n * NC * H * W or not prob.is_contiguous() or tuple(prob.shape[-3:]) != (NC, H, W)):
+        raise AotbError(f"tta_merge_batched: prob must be contiguous [{n}, {NC}, {H}, {W}], got {tuple(prob.shape)}")
+    arr = (ctypes.c_void_p * E)(*[t.data_ptr() for t in logits])
+    sizes = (ctypes.c_int * (2 * E))(*[int(v) for t in logits for v in t.shape[1:3]])
+    fl = (ctypes.c_int * E)(*[1 if f else 0 for f in flips])
+    ln = (ctypes.c_int * (n * E))(*[int(v) for r in lanes for v in r])
+    ob = (ctypes.c_int * n)(*[int(v) for v in obj_nums])
+    nl = _label_maps("tta_merge_batched new_labels", new_labels, n, H, W)
+    check(lib().aotb_tta_merge_batched_f32(arr, sizes, fl, E, ln, ob, n, NC, H, W, 1 if align_corners else 0, nl, _p(label),
+                                           _p(prob), _st(stream)), "aotb_tta_merge_batched_f32")
+    return label
+
+
+def tta_feedback_batched(logits, out, obj_nums, flips, output_size, align_corners, new_labels=None, stream=None):
+    """tta_feedback over the first len(flips) lanes of one multi-video decoder's output in one launch.  logits [lanes, h, w, NC]
+    (NHWC, lane k masked at obj_nums[k] as logits_postproc masks it) or None (background for every lane); out [>= n, Hi, Wi]
+    contiguous, lane k written to out[k]; new_labels: n [H, W] maps or None entries, at output_size.  Lane k's map is bit for
+    bit logits_postproc + tta_feedback on lane k."""
+    import ctypes
+    _chk(logits, out)
+    n = len(flips)
+    H, W = int(output_size[0]), int(output_size[1])
+    Hi, Wi = out.shape[-2:]
+    if n < 1 or not out.is_contiguous() or out.numel() < n * Hi * Wi:
+        raise AotbError(f"tta_feedback_batched: out must be contiguous [>= {n}, Hi, Wi], got {tuple(out.shape)}")
+    h = w = NC = 0
+    ob = None
+    if logits is not None:
+        if logits.dim() != 4 or not logits.is_contiguous() or logits.shape[0] < n:
+            raise AotbError(f"tta_feedback_batched: logits must be contiguous NHWC [>= {n}, h, w, NC], got "
+                            f"{tuple(logits.shape)}")
+        if obj_nums is None or len(obj_nums) != n:
+            raise AotbError(f"tta_feedback_batched: one object count per lane, got {obj_nums}")
+        h, w, NC = (int(v) for v in logits.shape[1:])
+        ob = (ctypes.c_int * n)(*[int(v) for v in obj_nums])
+    fl = (ctypes.c_int * n)(*[1 if f else 0 for f in flips])
+    nl = _label_maps("tta_feedback_batched new_labels", new_labels, n, H, W)
+    check(lib().aotb_tta_feedback_batched_f32(_p(logits), h, w, NC, n, ob, fl, nl, H, W, 1 if align_corners else 0, _p(out),
+                                              Hi, Wi, _st(stream)), "aotb_tta_feedback_batched_f32")
+    return out
+
+
 def separate_labels(mask, out, max_obj, stream=None):
     """mask: contiguous label map with HW elements; out [E, ...HW...] receives the per-engine renumbered label maps."""
     _chk(mask, out)

@@ -26,6 +26,24 @@ from .engine import _ENGINES, fork_join
 MAX_AUGS = 8        # aotb_tta_merge_f32 takes up to 8 logit maps
 
 
+def tta_augmentations(cfg, flip, multi_scale):
+    """The augmentations of a TTA engine -> (flip, scales, per-augmentation flip bits), scale-major with the unflipped one
+    first (FramePreprocessor's order).  flip / multi_scale default to cfg.TEST_FLIP / cfg.TEST_MULTISCALE.  Refuses
+    MODEL_USE_PREV_PROB and more than MAX_AUGS augmentations."""
+    if getattr(cfg, "MODEL_USE_PREV_PROB", False):
+        raise NotImplementedError(
+            "MODEL_USE_PREV_PROB with test-time augmentation has no reference behaviour to follow: "
+            "networks/managers/evaluator.py:438 reads current_prob before any assignment (its only assignment, :433, is "
+            "commented out), so the reference cannot run it")
+    flip = bool(getattr(cfg, "TEST_FLIP", False) if flip is None else flip)
+    scales = [float(s) for s in (getattr(cfg, "TEST_MULTISCALE", [1]) if multi_scale is None else multi_scale)]
+    flips = [f for _ in scales for f in ((False, True) if flip else (False,))]
+    if not 1 <= len(flips) <= MAX_AUGS:
+        raise ValueError(f"test-time augmentation runs 1 to {MAX_AUGS} augmentations, got {len(flips)} "
+                         f"({len(scales)} scales{' x 2 flips' if flip else ''})")
+    return flip, scales, flips
+
+
 class TTAInferEngine(nn.Module):
     def __init__(self, aot_model, gpu_id=0, long_term_mem_gap=9999, short_term_mem_skip=1, flip=None, multi_scale=None,
                  long_term_mem_max=None, precision=None, long_term_mem_policy=None):
@@ -36,19 +54,9 @@ class TTAInferEngine(nn.Module):
         engine's (see AOTEngine for all three)."""
         super().__init__()
         cfg = aot_model.cfg
-        if getattr(cfg, "MODEL_USE_PREV_PROB", False):
-            raise NotImplementedError(
-                "MODEL_USE_PREV_PROB with test-time augmentation has no reference behaviour to follow: "
-                "networks/managers/evaluator.py:438 reads current_prob before any assignment (its only assignment, :433, is "
-                "commented out), so the reference cannot run it")
         self.cfg = cfg
         self.AOT = aot_model
-        self.flip = bool(getattr(cfg, "TEST_FLIP", False) if flip is None else flip)
-        self.multi_scale = [float(s) for s in (getattr(cfg, "TEST_MULTISCALE", [1]) if multi_scale is None else multi_scale)]
-        self.flips = [f for _ in self.multi_scale for f in ((False, True) if self.flip else (False,))]
-        if not 1 <= len(self.flips) <= MAX_AUGS:
-            raise ValueError(f"test-time augmentation runs 1 to {MAX_AUGS} augmentations, got {len(self.flips)} "
-                             f"({len(self.multi_scale)} scales{' x 2 flips' if self.flip else ''})")
+        self.flip, self.multi_scale, self.flips = tta_augmentations(cfg, flip, multi_scale)
         cls = _ENGINES.get((cfg.MODEL_ENGINE, "eval"))
         if cls is None:
             raise NotImplementedError(f"no eval engine '{cfg.MODEL_ENGINE}'")

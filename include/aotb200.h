@@ -297,6 +297,25 @@ int aotb_tta_merge_f32(const float* const* logits, const int* sizes, const int* 
  * W-1-sx : sx], or 0 when new_label is null; out = n != 0 ? n : base. */
 int aotb_tta_feedback_f32(const float* logits, int h, int w, int NC, int H, int W, int align_corners, int flip,
                           const float* new_label, float* out, int Hi, int Wi, void* stream);
+/* aotb_tta_merge_f32 over n videos in one launch (32 per launch; more are chunked), reading each augmentation's logits straight
+ * from a multi-video decoder's output instead of aotb_logits_postproc_f32's maps (networks/managers/evaluator.py:332-369 per
+ * video, after networks/engines/aot_engine.py:367-378 per augmentation).  logits[e]: augmentation e's decoder output
+ * [lanes][h_e][w_e][NC] (NHWC, sizes[2e], sizes[2e+1]); video b reads lane lanes[b * n_augs + e] of it, where a channel above
+ * obj_nums[b] reads -1e10 at every bilinear tap, the value aotb_logits_postproc_f32 writes.  label [n][H][W]; pred_prob
+ * [n][NC][H][W] when not null; new_labels: n pointers to [H][W] overlays, or null, and any entry may be null.  Video b's label
+ * and prob are bit for bit aotb_logits_postproc_f32 (low-res, obj_nums[b]) on each of its lanes followed by
+ * aotb_tta_merge_f32. */
+int aotb_tta_merge_batched_f32(const float* const* logits, const int* sizes, const int* flips, int n_augs, const int* lanes,
+                               const int* obj_nums, int n, int NC, int H, int W, int align_corners,
+                               const float* const* new_labels, float* label, float* pred_prob, void* stream);
+/* aotb_tta_feedback_f32 over n_lanes lanes of one multi-video decoder's output in one launch (32 per launch; more are
+ * chunked).  logits: [n_lanes][h][w][NC] (NHWC), lane k masked at obj_nums[k] as aotb_logits_postproc_f32 masks it, or null
+ * (base = 0 for every lane, the first-frame and teacher-forced form; obj_nums may then be null).  flips[k]; new_labels: n_lanes
+ * pointers to [H][W] maps, or null, and any entry may be null.  out [n_lanes][Hi][Wi]: lane k's map is bit for bit
+ * aotb_logits_postproc_f32 + aotb_tta_feedback_f32 on lane k. */
+int aotb_tta_feedback_batched_f32(const float* logits, int h, int w, int NC, int n_lanes, const int* obj_nums,
+                                  const int* flips, const float* const* new_labels, int H, int W, int align_corners,
+                                  float* out, int Hi, int Wi, void* stream);
 
 /* Tensor-core long-term attention (wgmma + TMA), AOT head shape H x 32, split-fp16 ("fp16x2")
  * operands: every fp32 value x is stored as hi = fp16(x), lo = fp16(x - hi) in rows [hi(32) | lo(32)].
