@@ -517,6 +517,33 @@ __global__ void tta_feedback_batched_kernel(const float* __restrict__ lg, int h,
 // tensors, two concatenations, a product, a clamp and a logit (7 passes over E x 18 MB at 480p).
 struct AggArgs { const float* logits[8]; };
 
+// One output pixel of soft_logit_aggregation for the batched kernel: ld(e, c) is engine e's logit of channel c at the pixel;
+// emit.engine(e).fg(c, v) receives the merged logit of engine e's object c (c >= 1), emit.bg(v) the merged background.  It
+// performs soft_logit_aggregation_kernel's operations in the same order, so every merged logit is bit for bit the one-video
+// kernel's; that kernel keeps its own copy of them because inlining this body there changes its compiled code.
+template <int NC, class Load, class Emit>
+__device__ __forceinline__ void soft_logit_aggregation_pixel(const Load& ld, int E, Emit& emit) {
+    float bg = 1.f;
+    for (int e = 0; e < E; ++e) {
+        float v[NC];
+        float m = -INFINITY;
+#pragma unroll
+        for (int c = 0; c < NC; ++c) { v[c] = ld(e, c); m = fmaxf(m, v[c]); }
+        float sum = 0.f;
+#pragma unroll
+        for (int c = 0; c < NC; ++c) { v[c] = expf(v[c] - m); sum += v[c]; }
+        bg *= v[0] / sum;
+        auto o = emit.engine(e);
+#pragma unroll
+        for (int c = 1; c < NC; ++c) {
+            const float p = fminf(fmaxf(v[c] / sum, 1e-5f), 1.f - 1e-5f);
+            o.fg(c, logf(p / (1.f - p)));
+        }
+    }
+    const float p = fminf(fmaxf(bg, 1e-5f), 1.f - 1e-5f);
+    emit.bg(logf(p / (1.f - p)));
+}
+
 template <int NC>
 __global__ void soft_logit_aggregation_kernel(const AggArgs a, int E, float* __restrict__ out, int HW) {
     pdl_sync();
@@ -544,6 +571,83 @@ __global__ void soft_logit_aggregation_kernel(const AggArgs a, int E, float* __r
     }
 }
 
+// logits_upsample_kernel's value at one output pixel, read from one lane [h][w][NC] of a decoder output with
+// logits_mask_kernel's mask applied at every tap (a channel above obj reads -1e10).  The blend spells out the contraction nvcc
+// gives logits_upsample_kernel, fma(lx, v1, hx * v0) per row and fma(hy, row0, ly * row1) across rows, so every value is bit
+// for bit aotb_logits_postproc_f32's.
+__device__ __forceinline__ float upsample_nhwc(const float* __restrict__ b, int w, int NC, int c, int obj, int y0, int y1,
+                                               int x0, int x1, float ly, float lx) {
+    auto tap = [&](int y, int x) { return c > obj ? -1e10f : __ldg(b + ((y * w + x) * NC + c)); };   // a lane < 2^31
+    const float hy = 1.f - ly, hx = 1.f - lx;
+    const float r0 = __fmaf_rn(lx, tap(y0, x1), __fmul_rn(hx, tap(y0, x0)));
+    const float r1 = __fmaf_rn(lx, tap(y1, x1), __fmul_rn(hx, tap(y1, x0)));
+    return __fmaf_rn(hy, r0, __fmul_rn(ly, r1));
+}
+
+// soft_logit_aggregation over several videos of a multi-video pool, reading the decoder output [lanes][h][w][NC] directly:
+// video b = blockIdx.y aggregates its k[b] lanes in sub-engine order, each masked at its own object count and sampled at
+// [Ho][Wo] as aotb_logits_postproc_f32 does (upsample_nhwc; read unchanged when the size is [h][w]).  Writes the merged map out[b] [1 + k (NC - 1)][Ho][Wo] and / or label[b] [Ho][Wo], the map's first argmax; the
+// label compares the very values the map receives.
+constexpr int AGG_BATCH = 32;
+
+struct AggBatchArgs {
+    int lane[AGG_BATCH][8];
+    int obj[AGG_BATCH][8];
+    int k[AGG_BATCH];
+    float* out[AGG_BATCH];
+    float* label[AGG_BATCH];
+};
+
+template <int NC>
+struct AggBatchOut {
+    float* out;                 // null: label only
+    size_t total;
+    int i;
+    float best;
+    int bi;
+    struct Engine {
+        AggBatchOut& s;
+        int ch0;
+        __device__ __forceinline__ void fg(int c, float v) {
+            const int ch = ch0 + c - 1;
+            if (s.out) s.out[ch * s.total + s.i] = v;
+            if (v > s.best) { s.best = v; s.bi = ch; }
+        }
+    };
+    __device__ __forceinline__ Engine engine(int e) { return Engine{*this, 1 + e * (NC - 1)}; }
+    __device__ __forceinline__ void bg(float v) {
+        if (out) out[i] = v;
+        if (!(best > v)) bi = 0;          // channel 0 comes first: it wins a tie
+    }
+};
+
+template <int NC>
+__global__ void soft_logit_aggregation_batched_kernel(const float* __restrict__ lg, int h, int w, int Ho, int Wo, int align,
+                                                      const AggBatchArgs a) {
+    pdl_sync();
+    const int b = blockIdx.y;
+    const int E = a.k[b];
+    const int total = Ho * Wo;
+    const bool same = Ho == h && Wo == w;
+    const size_t lane = (size_t)h * w * NC;
+    float* label = a.label[b];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+        const int oy = i / Wo, ox = i - oy * Wo;
+        int y0, y1, x0, x1;
+        float ly, lx;
+        bl_src(oy, h, Ho, align, y0, y1, ly);
+        bl_src(ox, w, Wo, align, x0, x1, lx);
+        auto ld = [&](int e, int c) {
+            const float* base = lg + (size_t)a.lane[b][e] * lane;
+            const int obj = a.obj[b][e];
+            if (same) return c > obj ? -1e10f : __ldg(base + ((size_t)(oy * w + ox) * NC + c));
+            return upsample_nhwc(base, w, NC, c, obj, y0, y1, x0, x1, ly, lx);
+        };
+        AggBatchOut<NC> emit{a.out[b], (size_t)total, i, -INFINITY, 0};
+        soft_logit_aggregation_pixel<NC>(ld, E, emit);
+        if (label) label[i] = (float)emit.bi;
+    }
+}
 
 // separate_mask for label maps (aot_engine.py:515-533): engine e keeps ids [e*max_obj + 1, (e+1)*max_obj], renumbered from 1,
 // everything else becomes background.  One pass writes all E maps (the reference builds E boolean masks and 3 E temporaries).
@@ -554,6 +658,56 @@ __global__ void separate_labels_kernel(const float* __restrict__ mask, int E, in
         for (int e = 0; e < E; ++e) {
             const float lo = (float)(e * max_obj + 1), hi = (float)((e + 1) * max_obj);
             out[(size_t)e * HW + i] = (m >= lo && m <= hi) ? m - lo + 1.f : 0.f;
+        }
+    }
+}
+
+// separate_labels_kernel for the lanes of several videos: entry b = blockIdx.y writes out[b] = part[b]'s map of label[b].  The
+// per-element arithmetic is separate_labels_kernel's, which keeps its own copy so that its compiled code is unchanged.
+__device__ __forceinline__ float separate_label(float m, int e, int max_obj) {
+    const float lo = (float)(e * max_obj + 1), hi = (float)((e + 1) * max_obj);
+    return (m >= lo && m <= hi) ? m - lo + 1.f : 0.f;
+}
+
+constexpr int SEP_BATCH = 32;
+
+struct SepBatchArgs {
+    const float* label[SEP_BATCH];
+    float* out[SEP_BATCH];
+    int part[SEP_BATCH];
+};
+
+__global__ void separate_labels_batched_kernel(const SepBatchArgs a, int max_obj, int HW) {
+    pdl_sync();
+    const int b = blockIdx.y;
+    const float* __restrict__ mask = a.label[b];
+    float* __restrict__ out = a.out[b];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x)
+        out[i] = separate_label(mask[i], a.part[b], max_obj);
+}
+
+// Gather of up to four per-video maps into lane order: for every map j, lane l = blockIdx.y copies video lane_video[l]'s
+// n4[j] float4s from src[j] into its own rows of dst[j].  A table entry outside [0, n_videos) copies nothing.
+struct LaneGatherArgs {
+    const float* src[4];
+    float* dst[4];
+    int n4[4];
+};
+
+__global__ void __launch_bounds__(256) lane_gather_kernel(const LaneGatherArgs a, int n_maps, const int* __restrict__ lane_video,
+                                                          int n_videos) {
+    pdl_sync();
+    const int l = blockIdx.y;
+    const int v = lane_video[l];
+    if (v < 0 || v >= n_videos) return;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        if (j < n_maps) {
+            const size_t n4 = a.n4[j];
+            const float4* __restrict__ s = reinterpret_cast<const float4*>(a.src[j]) + (size_t)v * n4;
+            float4* __restrict__ d = reinterpret_cast<float4*>(a.dst[j]) + (size_t)l * n4;
+            for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x)
+                d[i] = __ldg(s + i);
         }
     }
 }
@@ -866,6 +1020,86 @@ extern "C" int aotb_separate_labels_f32(const float* mask, int n_engines, int ma
     if (g > 132 * 8) g = 132 * 8;
     launch(separate_labels_kernel, dim3(g), dim3(256), 0, (cudaStream_t)stream, mask, n_engines, max_obj, out, HW);
     return check_launch("aotb_separate_labels_f32");
+}
+
+// logits: decoder output [lanes][h][w][NC] (NHWC); video b's k[b] = lane_ptr[b + 1] - lane_ptr[b] lanes are
+// lanes[lane_ptr[b] ..], with object counts obj_nums[lane_ptr[b] ..]; out / label: n_videos pointers or null arrays.
+extern "C" int aotb_soft_logit_aggregation_batched_f32(const float* logits, int h, int w, int NC, const int* lane_ptr,
+                                                       const int* lanes, const int* obj_nums, int n_videos, int max_obj,
+                                                       int Ho, int Wo, int align_corners, float* const* out,
+                                                       float* const* label, void* stream) {
+    AOTB_REQUIRE(logits && lane_ptr && lanes && obj_nums && n_videos > 0 && h > 0 && w > 0 && Ho > 0 && Wo > 0 && (out || label),
+                 "aotb_soft_logit_aggregation_batched_f32: bad args");
+    AOTB_REQUIRE(max_obj == 10 && NC == 11, "aotb_soft_logit_aggregation_batched_f32: built for MODEL_MAX_OBJ_NUM = 10 (got "
+                 "max_obj %d, NC %d)", max_obj, NC);
+    AOTB_REQUIRE((size_t)h * w * NC < (1u << 31), "aotb_soft_logit_aggregation_batched_f32: lane too large");
+    const size_t plane = (size_t)Ho * Wo;
+    AggBatchArgs a;
+    int launches = 0;
+    for (int v0 = 0; v0 < n_videos; v0 += AGG_BATCH, ++launches) {
+        const int nb = n_videos - v0 < AGG_BATCH ? n_videos - v0 : AGG_BATCH;
+        for (int b = 0; b < nb; ++b) {
+            const int p = lane_ptr[v0 + b], k = lane_ptr[v0 + b + 1] - p;
+            AOTB_REQUIRE(k >= 1 && k <= 8, "aotb_soft_logit_aggregation_batched_f32: video %d: 1 to 8 lanes (got %d)", v0 + b, k);
+            for (int e = 0; e < 8; ++e) {
+                a.lane[b][e] = e < k ? lanes[p + e] : 0;
+                a.obj[b][e] = e < k ? obj_nums[p + e] : 0;
+                AOTB_REQUIRE(a.lane[b][e] >= 0, "aotb_soft_logit_aggregation_batched_f32: video %d: negative lane", v0 + b);
+            }
+            a.k[b] = k;
+            a.out[b] = out ? out[v0 + b] : nullptr;
+            a.label[b] = label ? label[v0 + b] : nullptr;
+            AOTB_REQUIRE(a.out[b] || a.label[b], "aotb_soft_logit_aggregation_batched_f32: video %d: no output", v0 + b);
+        }
+        int g = cdiv((int)plane, 256);
+        if (g > 132 * 8) g = 132 * 8;
+        launch(soft_logit_aggregation_batched_kernel<11>, dim3(g, nb), dim3(256), 0, (cudaStream_t)stream, logits, h, w, Ho, Wo,
+               align_corners, a);
+    }
+    return check_launch("aotb_soft_logit_aggregation_batched_f32", launches);
+}
+
+extern "C" int aotb_separate_labels_batched_f32(const float* const* labels, const int* parts, int n, int max_obj,
+                                                float* const* out, int HW, void* stream) {
+    AOTB_REQUIRE(labels && parts && out && n > 0 && max_obj >= 1 && HW > 0, "aotb_separate_labels_batched_f32: bad args");
+    SepBatchArgs a;
+    int g = cdiv(HW, 256);
+    if (g > 132 * 8) g = 132 * 8;
+    int launches = 0;
+    for (int b0 = 0; b0 < n; b0 += SEP_BATCH, ++launches) {
+        const int nb = n - b0 < SEP_BATCH ? n - b0 : SEP_BATCH;
+        for (int b = 0; b < nb; ++b) {
+            a.label[b] = labels[b0 + b];
+            a.out[b] = out[b0 + b];
+            a.part[b] = parts[b0 + b];
+            AOTB_REQUIRE(a.label[b] && a.out[b] && a.part[b] >= 0, "aotb_separate_labels_batched_f32: entry %d: bad map or part",
+                         b0 + b);
+        }
+        launch(separate_labels_batched_kernel, dim3(g, nb), dim3(256), 0, (cudaStream_t)stream, a, max_obj, HW);
+    }
+    return check_launch("aotb_separate_labels_batched_f32", launches);
+}
+
+extern "C" int aotb_lane_gather_f32(const float* const* src, float* const* dst, const int* n_floats, int n_maps,
+                                    const int* lane_video, int n_lanes, int n_videos, void* stream) {
+    AOTB_REQUIRE(src && dst && n_floats && lane_video && n_maps >= 1 && n_maps <= 4 && n_lanes >= 1 && n_lanes <= 65535 &&
+                 n_videos >= 1, "aotb_lane_gather_f32: bad args");
+    LaneGatherArgs a;
+    int most = 0;
+    for (int j = 0; j < 4; ++j) {
+        const bool live = j < n_maps;
+        a.src[j] = live ? src[j] : nullptr;
+        a.dst[j] = live ? dst[j] : nullptr;
+        a.n4[j] = live ? n_floats[j] / 4 : 0;
+        AOTB_REQUIRE(!live || (a.src[j] && a.dst[j] && n_floats[j] > 0 && n_floats[j] % 4 == 0 &&
+                               ((uintptr_t)a.src[j] | (uintptr_t)a.dst[j]) % 16 == 0),
+                     "aotb_lane_gather_f32: map %d: null, unaligned or not a multiple of 4 floats", j);
+        if (a.n4[j] > most) most = a.n4[j];
+    }
+    int g = cdiv(most, 256);
+    if (g > 132 * 4) g = 132 * 4;
+    launch(lane_gather_kernel, dim3(g, n_lanes), dim3(256), 0, (cudaStream_t)stream, a, n_maps, lane_video, n_videos);
+    return check_launch("aotb_lane_gather_f32");
 }
 
 extern "C" int aotb_bank_append_f32(const float* src, int lds, float* bank, int ldb, int rows, int cols, int offset,

@@ -145,7 +145,7 @@ class MultiVideoTTAInferEngine:
         self._check_lane_imgs(imgs)
         H, W = int(label.shape[-2]), int(label.shape[-1])
         self._check_size((H, W))
-        obj = self.pools[0]._check_objs(obj_nums)
+        obj = self._check_objs(obj_nums)
         lab = self._label_map(label, H, W)
         v = dict(vid=self._next_vid, obj=obj, lanes=[])
         try:
@@ -169,6 +169,15 @@ class MultiVideoTTAInferEngine:
         self._size = (H, W)
         self._trim_encoders()
         return v["vid"]
+
+    def _check_objs(self, obj_nums):
+        if isinstance(obj_nums, (list, tuple)):
+            obj_nums = obj_nums[0]
+        obj = int(obj_nums)
+        if obj > self.max_obj_num:
+            raise NotImplementedError(f"{type(self).__name__} propagates at most {self.max_obj_num} objects per video (one "
+                                      f"ID bank per augmentation), got {obj}")
+        return obj
 
     def close_video(self, vid):
         """Close every lane of the video (each pool compacts its own slots)."""

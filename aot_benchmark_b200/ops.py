@@ -796,6 +796,110 @@ def separate_labels(mask, out, max_obj, stream=None):
     return out
 
 
+def soft_logit_aggregation_batched(logits, lanes, obj_nums, align_corners, out=None, labels=None, max_obj=10, stream=None):
+    """soft_logit_aggregation for n videos of a multi-video pool in one launch, reading its decoder output logits [lanes, h, w,
+    1 + max_obj] (NHWC, contiguous) directly.  lanes [n][k_b] (1 <= k_b <= 8): video b's lanes in sub-engine order; obj_nums
+    [n][k_b]: their object counts, ids above which are masked as logits_postproc masks them.  out: n contiguous maps [1 +
+    k_b max_obj, Ho, Wo] (leading dims of size 1) or None; labels: n contiguous [Ho, Wo] maps or None (entries may be None, but
+    not both for one video).  Video b's map is bit for bit logits_postproc (at [Ho, Wo]) on each of its lanes followed by
+    soft_logit_aggregation, its label the first argmax of that map."""
+    import ctypes
+    n = len(lanes)
+    outs = [None] * n if out is None else list(out)
+    labs = [None] * n if labels is None else list(labels)
+    _chk(logits, *[t for t in outs + labs if t is not None])
+    if n < 1 or len(obj_nums) != n or len(outs) != n or len(labs) != n:
+        raise AotbError(f"soft_logit_aggregation_batched: lanes, obj_nums, out and labels need one entry per video, got "
+                        f"{n}, {len(obj_nums)}, {len(outs)}, {len(labs)}")
+    if logits.dim() != 4 or not logits.is_contiguous() or logits.shape[-1] != 1 + max_obj:
+        raise AotbError(f"soft_logit_aggregation_batched: logits must be contiguous NHWC [lanes, h, w, {1 + max_obj}], got "
+                        f"{tuple(logits.shape)}")
+    L, h, w, NC = (int(v) for v in logits.shape)
+    size = None
+    for b in range(n):
+        k = len(lanes[b])
+        if not 1 <= k <= 8 or len(obj_nums[b]) != k or any(not 0 <= int(l) < L for l in lanes[b]):
+            raise AotbError(f"soft_logit_aggregation_batched: video {b}: 1 to 8 lanes in [0, {L}) with one object count each, "
+                            f"got lanes {lanes[b]}, obj_nums {obj_nums[b]}")
+        if outs[b] is None and labs[b] is None:
+            raise AotbError(f"soft_logit_aggregation_batched: video {b}: no output")
+        for t, ch in ((outs[b], 1 + k * max_obj), (labs[b], None)):
+            if t is None:
+                continue
+            s = tuple(int(v) for v in t.shape[-2:])
+            size = size or s
+            lead = t.numel() // (s[0] * s[1])
+            if s != size or not t.is_contiguous() or (ch is None and lead != 1) or \
+                    (ch is not None and (t.dim() < 3 or t.shape[-3] != ch or lead != ch)):
+                raise AotbError(f"soft_logit_aggregation_batched: video {b}: need contiguous {'label' if ch is None else ch} "
+                                f"maps of one size {size}, got {tuple(t.shape)}")
+    ptr = [0]
+    for r in lanes:
+        ptr.append(ptr[-1] + len(r))
+    lp = (ctypes.c_int * (n + 1))(*ptr)
+    ln = (ctypes.c_int * ptr[-1])(*[int(v) for r in lanes for v in r])
+    ob = (ctypes.c_int * ptr[-1])(*[int(v) for r in obj_nums for v in r])
+    op = None if out is None else (ctypes.c_void_p * n)(*[_p(t) for t in outs])
+    lb = None if labels is None else (ctypes.c_void_p * n)(*[_p(t) for t in labs])
+    check(lib().aotb_soft_logit_aggregation_batched_f32(_p(logits), h, w, NC, lp, ln, ob, n, int(max_obj), size[0], size[1],
+                                                        1 if align_corners else 0, op, lb, _st(stream)),
+          "aotb_soft_logit_aggregation_batched_f32")
+    return out, labels
+
+
+def separate_labels_batched(labels, parts, out, max_obj=10, stream=None):
+    """separate_labels for n lanes in one launch: out[b] (contiguous, HW elements) = labels[b]'s map for sub-engine parts[b]
+    (ids (parts[b] max_obj, (parts[b] + 1) max_obj] renumbered from 1, everything else 0); labels[b] contiguous fp32 with the
+    same HW elements, and an entry may repeat.  Bit for bit row parts[b] of separate_labels on labels[b]."""
+    import ctypes
+    n = len(labels)
+    _chk(*labels, *out)
+    if n < 1 or len(parts) != n or len(out) != n:
+        raise AotbError(f"separate_labels_batched: one part and one output per label map, got {n}, {len(parts)}, {len(out)}")
+    HW = labels[0].numel()
+    for t in list(labels) + list(out):
+        if t.numel() != HW or not t.is_contiguous() or t.dtype != torch.float32:
+            raise AotbError(f"separate_labels_batched: every map must be contiguous fp32 with {HW} elements, got "
+                            f"{tuple(t.shape)} {t.dtype}")
+    if any(int(p) < 0 for p in parts):
+        raise AotbError(f"separate_labels_batched: negative part in {parts}")
+    lb = (ctypes.c_void_p * n)(*[_p(t) for t in labels])
+    op = (ctypes.c_void_p * n)(*[_p(t) for t in out])
+    pt = (ctypes.c_int * n)(*[int(p) for p in parts])
+    check(lib().aotb_separate_labels_batched_f32(lb, pt, n, int(max_obj), op, HW, _st(stream)),
+          "aotb_separate_labels_batched_f32")
+    return out
+
+
+def lane_gather(src, dst, lane_video, n_lanes, stream=None):
+    """Gather up to 4 per-video maps into lane order in one launch: dst[j][l] = src[j][lane_video[l]] for l < n_lanes.  src[j]
+    [videos, ...] and dst[j] [>= n_lanes, ...] contiguous fp32 with one row size (a multiple of 4 floats); lane_video: int32
+    device tensor [>= n_lanes] read at run time (a captured launch follows its contents), an entry outside [0, videos) copies
+    nothing."""
+    import ctypes
+    _chk(*src, *dst)
+    m = len(src)
+    if not 1 <= m <= 4 or len(dst) != m:
+        raise AotbError(f"lane_gather: 1 to 4 maps with one destination each, got {m} and {len(dst)}")
+    if not lane_video.is_cuda or lane_video.dtype != torch.int32 or not lane_video.is_contiguous() \
+            or lane_video.numel() < n_lanes or n_lanes < 1:
+        raise AotbError(f"lane_gather: lane_video must be a contiguous int32 tensor of >= {n_lanes} >= 1 entries")
+    nv = int(src[0].shape[0])
+    rows = []
+    for s, d in zip(src, dst):
+        r = s[0].numel() if s.shape[0] else 0
+        if s.dtype != torch.float32 or d.dtype != torch.float32 or not s.is_contiguous() or not d.is_contiguous() \
+                or s.shape[0] != nv or d.shape[0] < n_lanes or d[0].numel() != r or r % 4:
+            raise AotbError(f"lane_gather: need contiguous fp32 src [{nv}, ...] and dst [>= {n_lanes}, ...] with one row size "
+                            f"(a multiple of 4), got {tuple(s.shape)} and {tuple(d.shape)}")
+        rows.append(r)
+    sp = (ctypes.c_void_p * m)(*[_p(t) for t in src])
+    dp = (ctypes.c_void_p * m)(*[_p(t) for t in dst])
+    nf = (ctypes.c_int * m)(*rows)
+    check(lib().aotb_lane_gather_f32(sp, dp, nf, m, _p(lane_video), int(n_lanes), nv, _st(stream)), "aotb_lane_gather_f32")
+    return dst
+
+
 def preprocess_bgr_u8(img_u8, out, taps=None, flip=False, stream=None):
     """img_u8 uint8 [H, W, 3] (device); out fp32 [1, 3, Ho, Wo]; taps = (ix, cx, iy, cy) device tables or None (same size)."""
     if img_u8.dtype != torch.uint8 or not img_u8.is_cuda or not img_u8.is_contiguous() or img_u8.dim() != 3 or img_u8.shape[2] != 3:

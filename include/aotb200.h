@@ -272,6 +272,27 @@ int aotb_soft_logit_aggregation_f32(const float* const* logits, int n_engines, i
 /* networks/engines/aot_engine.py:515-533 (AOTInferEngine.separate_mask, label-map form): out[e][i] = mask[i] - e*max_obj if
  * e*max_obj < mask[i] <= (e+1)*max_obj else 0, for e in [0, n_engines). */
 int aotb_separate_labels_f32(const float* mask, int n_engines, int max_obj, float* out, int HW, void* stream);
+/* The multi-video engines' ID-bank lanes (a lane is the batched counterpart of one sub-engine; lane e of a video carries its ids
+ * 10e+1 .. 10e+10).  The three arrays of pointers, the counts and the CSR tables below are host memory. */
+/* aotb_soft_logit_aggregation_f32 for n_videos videos in one launch (32 per launch; more are chunked), reading a multi-video
+ * decoder's output logits [lanes][h][w][NC] (NHWC, NC = 1 + max_obj = 11) directly: video b's k = lane_ptr[b+1] - lane_ptr[b]
+ * (1..8) lanes are lanes[lane_ptr[b] ..] in sub-engine order, lane e masked above obj_nums[lane_ptr[b] + e] with -1e10 at
+ * every bilinear tap and sampled at [Ho][Wo] (read unchanged when that is [h][w]).  out[b] [1 + k max_obj][Ho][Wo] receives the
+ * merged logits and label[b] [Ho][Wo] their first argmax; either array, or any entry, may be null, not both for one video.
+ * Bit for bit aotb_logits_postproc_f32 on each lane followed by aotb_soft_logit_aggregation_f32. */
+int aotb_soft_logit_aggregation_batched_f32(const float* logits, int h, int w, int NC, const int* lane_ptr, const int* lanes,
+                                            const int* obj_nums, int n_videos, int max_obj, int Ho, int Wo, int align_corners,
+                                            float* const* out, float* const* label, void* stream);
+/* aotb_separate_labels_f32 for n lanes in one launch (32 per launch; more are chunked): out[b] [HW] = labels[b] [HW] separated
+ * for sub-engine parts[b], bit for bit row parts[b] of aotb_separate_labels_f32 on labels[b]. */
+int aotb_separate_labels_batched_f32(const float* const* labels, const int* parts, int n, int max_obj, float* const* out,
+                                     int HW, void* stream);
+/* Up to 4 per-video maps gathered into lane order in one launch: for map j, lane l's n_floats[j] floats of dst[j]
+ * [n_lanes][n_floats[j]] = video lane_video[l]'s of src[j] [n_videos][n_floats[j]].  lane_video is device memory (n_lanes
+ * ints), so a captured launch follows a table rewritten before its replay; an entry outside [0, n_videos) copies nothing.
+ * n_floats[j] must be a multiple of 4 and the maps 16-byte aligned. */
+int aotb_lane_gather_f32(const float* const* src, float* const* dst, const int* n_floats, int n_maps, const int* lane_video,
+                         int n_lanes, int n_videos, void* stream);
 /* Frame input side (SURVEY 8 f.3): dataloaders/eval_datasets.py:60-61 + dataloaders/video_transforms.py:594-715 (MultiRestrictSize's
  * cv2.resize(INTER_CUBIC) of the float image, MultiToTensor's / 255, - mean, / std, HWC -> CHW) on the uint8 frame in one pass.
  * img uint8 [H][W][3]; ix / cx [Wo][4] and iy / cy [Ho][4] = clamped tap indices and Keys-cubic (A = -0.75) weights per output
